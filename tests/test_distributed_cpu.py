@@ -3,7 +3,9 @@
 prefix offsets, rebase amounts, bit positions) and the semantics of every push job.  The shards are decoded by the host
 emulation (tests/emu) and each rank applies its jobs to a zeroed copy of the gathered arena; a bitwise-OR reduce to the
 leader stands in for the NVLink stores (the ranks' pushes touch disjoint bytes except for OR-merged bitmap seams).
-The NCCL + CUDA IPC + push-kernel path itself is exercised by tests/test_gpu_gather.py."""
+These byte-wise restatements check the plan, not gather_push_kernel's word-level code: that kernel is tested in
+tests/test_gpu_gather.py on one GPU (every rank a separate result on cuda:0) against the oracle, and the NCCL + CUDA
+IPC path there with two GPUs."""
 import os
 import random
 
