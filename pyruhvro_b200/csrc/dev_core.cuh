@@ -49,7 +49,64 @@ __device__ __forceinline__ uint32_t lds_u32(uint32_t a) { uint32_t v; asm("ld.sh
 __device__ __forceinline__ uint64_t lds_u64(uint32_t a) { uint64_t v; asm("ld.shared.u64 %0, [%1];" : "=l"(v) : "r"(a)); return v; }
 __device__ __forceinline__ void sts_u32(uint32_t a, uint32_t v) { asm volatile("st.shared.u32 [%0], %1;" ::"r"(a), "r"(v) : "memory"); }
 __device__ __forceinline__ void reds_or_u32(uint32_t a, uint32_t v) { asm volatile("red.shared.or.b32 [%0], %1;" ::"r"(a), "r"(v) : "memory"); }
+__device__ __forceinline__ uint32_t lds_u8v(uint32_t a) { uint32_t v; asm volatile("ld.shared.u8 %0, [%1];" : "=r"(v) : "r"(a) : "memory"); return v; }
+__device__ __forceinline__ void sts_u8(uint32_t a, uint32_t v) { asm volatile("st.shared.u8 [%0], %1;" ::"r"(a), "r"(v) : "memory"); }
 #endif
+
+// ---- warp collectives of the item-parallel list emit (generated walkers) ----------------------------------------
+// On the host, the item-parallel emit runs only under a lock-step warp emulation (tests/emu/warp_emu.cpp) that installs
+// itself here: it holds the item-position table and runs the 32 lanes of a warp as coroutines that meet at every
+// collective, where each lane hands in one value and gets the whole warp's 32.  Without it (the per-lane host emulation)
+// the generated walkers keep their per-lane item loops.
+#if !defined(__CUDA_ARCH__)
+struct HostWarpEmu {
+    uint8_t* items;                                       // the tile's item-position table
+    const uint32_t* (*exchange)(uint32_t lane, uint32_t v);
+};
+// (internal linkage: an inline function's static would be one object across every emulation library in the process)
+static inline HostWarpEmu*& host_warp_emu() { static HostWarpEmu* e = nullptr; return e; }
+#endif
+// Whether the item-parallel emit (and the count walk's item positions) are in use: always on the device.
+RV_HD bool item_parallel_on() {
+#if defined(__CUDA_ARCH__)
+    return true;
+#else
+    return host_warp_emu() != nullptr;
+#endif
+}
+RV_HD uint32_t warp_shfl(uint32_t v, uint32_t src, uint32_t lane) {
+#if defined(__CUDA_ARCH__)
+    (void)lane;
+    return __shfl_sync(0xFFFFFFFFu, v, int(src));
+#else
+    return host_warp_emu()->exchange(lane, v)[src];
+#endif
+}
+RV_HD bool warp_any(bool pred, uint32_t lane) {
+#if defined(__CUDA_ARCH__)
+    (void)lane;
+    return __any_sync(0xFFFFFFFFu, pred);
+#else
+    const uint32_t* a = host_warp_emu()->exchange(lane, pred ? 1u : 0u);
+    for (int i = 0; i < 32; ++i) if (a[i]) return true;
+    return false;
+#endif
+}
+// inclusive prefix sum over the warp's lanes
+RV_HD uint32_t warp_scan_incl(uint32_t v, uint32_t lane) {
+#if defined(__CUDA_ARCH__)
+    for (int d = 1; d < 32; d <<= 1) {
+        const uint32_t u = __shfl_up_sync(0xFFFFFFFFu, v, d);
+        if (int(lane) >= d) v += u;
+    }
+    return v;
+#else
+    const uint32_t* a = host_warp_emu()->exchange(lane, v);
+    uint32_t s = 0;
+    for (uint32_t i = 0; i <= lane; ++i) s += a[i];
+    return s;
+#endif
+}
 
 // SM = the record's bytes were staged into shared memory (device) — the FAST flavour.
 template <bool SM>
@@ -74,7 +131,27 @@ struct WalkCtx {
     uint32_t row0;         // chunk-local row of this record
     bool in_range;         // the lane owns a record
     bool store_word;       // space-0 bitmaps: this lane stores the warp's ballot word
+    uint32_t items_saddr;  // fast (device): shared-space address of the item-position table (dev_types.h kItemSlots)
 };
+
+// Entry `i` of the item-position table, written by the FAST count walk and read by the item-parallel emit.
+template <class C>
+RV_HD void itab_put(C& c, uint32_t i, uint32_t v) {
+#if defined(__CUDA_ARCH__)
+    sts_u8(c.items_saddr + i, v);
+#else
+    host_warp_emu()->items[i] = uint8_t(v);
+#endif
+}
+template <class C>
+RV_HD uint32_t itab_get(const C& c, uint32_t i) {
+#if defined(__CUDA_ARCH__)
+    return lds_u8v(c.items_saddr + i);
+#else
+    (void)c;
+    return host_warp_emu()->items[i];
+#endif
+}
 
 // PRECISE: records the first error of the record and parks the cursor at the record's end, so every later
 // read of this lane fails on its own (EOF) without the walkers re-checking c.err at each node.

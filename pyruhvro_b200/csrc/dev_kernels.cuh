@@ -21,7 +21,8 @@
 //   exact-size arena.  p.count_only (the first call on a schema) skips every emit.
 //
 // Shared-memory map (dynamic, rv_smem; smem_map() in dev_types.h):
-//   [nodes n_nodes*32][ttot (S+1)*4][tbase S*4][adj S*4][flags 16][mbar 8][ptrs n_slots*8][cur S*256*4 (interpreter)]
+//   [nodes n_nodes*32][ttot (S+1)*4][tbase S*4][adj S*4][flags 16][mbar 8][ptrs n_slots*8][item positions (generated walkers)]
+//   [cur S*256*4 (interpreter)]
 //   [in: smem_data_cap + pad][stage: smem_stage_cap]        (register-cursor walkers: the scan area overlays `stage`)
 #pragma once
 #include "dev_core.cuh"
@@ -230,6 +231,7 @@ __device__ __forceinline__ int64_t init_ctx(C& c, const DecodeParams& p, const T
     c.stage_on = false;
     c.stage_saddr = s0 + m.stage;
     c.adj_saddr = s0 + m.adj;
+    c.items_saddr = s0 + m.items;
     c.in_range = tid < t.nrec;
     c.row0 = uint32_t(t.local_tile) * kBlock + tid;
     c.store_word = (tid & 31) == 0 && int64_t(c.row0) < t.chunk_len;
@@ -406,7 +408,7 @@ __device__ __forceinline__ void stage_write_out(const DecodeParams& p, const Sme
 template <class W>
 __device__ __forceinline__ void fused_body(const DecodeParams& p, const int tile_id) {
     const Tile t = tile_of(p, tile_id);
-    const SmemMap m = smem_map(p.n_nodes, p.n_streams, p.n_slots, p.smem_data_cap, p.smem_stage_cap, W::kRegCursors);
+    const SmemMap m = smem_map(p.n_nodes, p.n_streams, p.n_slots, p.smem_data_cap, p.smem_stage_cap, W::kRegCursors, W::kItemBytes);
     typename W::Cur q;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const TileWindow w = stage_in<W>(p, t, tile_id, m);

@@ -149,18 +149,33 @@ struct DecodeParams {
 // the staged window is followed by this many readable bytes.
 constexpr uint32_t kWindowPad = 64;
 
+// Item-position table of the item-parallel list/map emit (generated walkers, jit.cpp).  For each top-level list/map
+// whose items are walked (list index L) and each lane, the FAST count walk stores kItemEntries bytes, as offsets from
+// where the list starts in the record: the starts of its first kItemSlots items, the position after the terminating
+// block, and the item count — kItemSeq when the lane has more than kItemSlots items or the list spans more than 255
+// bytes, which makes its warp emit that list with the per-lane loop.  Entry (L, j) of lane t is byte
+// (L * kItemEntries + j) * kBlock + t.  (One byte per entry: 1.5 KiB per list keeps the Kafka plan at three CTAs per SM.)
+constexpr int kItemSlots = 4;
+constexpr int kItemEntries = kItemSlots + 2;
+constexpr uint32_t kItemSeq = 0xFFu;
+#if defined(__CUDACC__)
+__host__ __device__
+#endif
+constexpr uint32_t item_table_bytes(int n_lists) { return uint32_t(n_lists) * uint32_t(kItemEntries) * uint32_t(kBlock); }
+
 // Dynamic shared-memory map of a decode CTA (byte offsets inside the CTA's shared memory):
-//   [nodes n_nodes*32][ttot (S+1)*4][tbase S*4][adj S*4][flags 16][mbar 8][ptrs n_slots*8][cur S*kBlock*4][in: data_cap+pad][stage: stage_cap]
+//   [nodes n_nodes*32][ttot (S+1)*4][tbase S*4][adj S*4][flags 16][mbar 8][ptrs n_slots*8][items item_bytes]
+//   [cur S*kBlock*4][in: data_cap+pad][stage: stage_cap]
 // alias_cur (walkers that keep their cursors in registers): the scan area `cur` overlays the Utf8 staging area
 // (it is dead before the first staged byte is written) and costs no extra shared memory.
 struct SmemMap {
-    uint32_t nodes, ttot, tbase, adj, flags, mbar, ptrs, cur, in, stage, total;
+    uint32_t nodes, ttot, tbase, adj, flags, mbar, ptrs, items, cur, in, stage, total;
 };
 
 #if defined(__CUDACC__)
 __host__ __device__
 #endif
-inline SmemMap smem_map(int n_nodes, int n_streams, int n_slots, uint32_t data_cap, uint32_t stage_cap, bool alias_cur) {
+inline SmemMap smem_map(int n_nodes, int n_streams, int n_slots, uint32_t data_cap, uint32_t stage_cap, bool alias_cur, uint32_t item_bytes) {
     SmemMap m;
     m.nodes = 0;
     m.ttot = uint32_t(n_nodes) * 32u;
@@ -169,7 +184,8 @@ inline SmemMap smem_map(int n_nodes, int n_streams, int n_slots, uint32_t data_c
     m.flags = (m.adj + uint32_t(n_streams) * 4u + 15u) & ~15u;
     m.mbar = m.flags + 16u;  // mbarrier of the bulk-copy staging (8 bytes)
     m.ptrs = m.mbar + 16u;
-    m.cur = (m.ptrs + uint32_t(n_slots) * 8u + 15u) & ~15u;
+    m.items = (m.ptrs + uint32_t(n_slots) * 8u + 15u) & ~15u;
+    m.cur = (m.items + item_bytes + 15u) & ~15u;
     const uint32_t cur_bytes = uint32_t(n_streams) * kBlock * 4u;
     m.in = alias_cur ? m.cur : ((m.cur + cur_bytes + 15u) & ~15u);
     m.stage = (m.in + data_cap + kWindowPad + 15u) & ~15u;

@@ -707,7 +707,10 @@ rv_status decode_on_device(rv_schema* s, const uint8_t* d_data, const int64_t* d
     // ---- shared-memory windows: [fixed tables][input window (+pad)][Utf8 staging / scan area] ----------
     const size_t limit = 227 * 1024;
     const size_t cur_bytes = size_t(S) * kBlock * 4;
-    const size_t fixed = smem_map(plan_nodes, S, n_slots, 0, 0, use_jit).stage;  // everything but the two windows (incl. the pad)
+    // the generated walker's item-position table is one of the fixed tables: it comes out of the two windows' room
+    // (configure below gives up the windows' margin where that keeps a CTA per SM)
+    const uint32_t item_bytes = use_jit ? item_table_bytes(item_parallel_lists(plan)) : 0u;
+    const size_t fixed = smem_map(plan_nodes, S, n_slots, 0, 0, use_jit, item_bytes).stage;  // everything but the two windows (incl. the pad)
     if (fixed + (use_jit ? cur_bytes : 0) + 2048 > limit) return fail(RV_ERR_SCHEMA, "schema too wide for the shared-memory cursor table");
     size_t smem_bytes = 0;
     auto configure = [&](const SchemaStats& st_) {  // re-evaluated per pass: a measuring pass teaches the next one
@@ -720,7 +723,7 @@ rv_status decode_on_device(rv_schema* s, const uint8_t* d_data, const int64_t* d
         want_in = std::max<size_t>(align_up(want_in, 64), 2048);
         const size_t room = (limit - fixed - 64) & ~size_t(15);
         const size_t min_stage = use_jit ? align_up(cur_bytes, 16) : 0;
-        const size_t cap_in = std::min(want_in, room - std::min(room, min_stage));
+        size_t cap_in = std::min(want_in, room - std::min(room, min_stage));
         size_t cap_stage = 0;
         if (p.n_utf8 > 0) {
             // a tile's share of the Utf8 bytes: the largest seen (+6%), else everything the window could hold
@@ -734,10 +737,25 @@ rv_status decode_on_device(rv_schema* s, const uint8_t* d_data, const int64_t* d
         }
         cap_stage = std::max(cap_stage, min_stage);
         if (cap_in + cap_stage > room) cap_stage = std::max<size_t>(min_stage, (room - cap_in) & ~size_t(15));
+        // The windows carry a margin over the largest tile seen (1/16 each).  Where that margin is all that keeps the SM
+        // from holding one more CTA — Kafka: windows + the item-position table just above a third of the SM — it is
+        // given up, 64 bytes at a time, down to the largest tile seen; otherwise the windows stay as they are.
+        if (hints.max_span < 0 && (st_.max_span || st_.max_utf8)) {
+            auto ctas = [&](size_t in_b, size_t st_b) { return (228 * 1024) / (smem_map(plan_nodes, S, n_slots, uint32_t(in_b), uint32_t(st_b), use_jit, item_bytes).total + 1024); };
+            const size_t floor_in = st_.max_span ? std::min(cap_in, std::max<size_t>(align_up(size_t(st_.max_span) + 48, 64), 2048)) : cap_in;
+            const size_t floor_stage = st_.max_utf8 ? std::min(cap_stage, std::max(min_stage, size_t(align_up(size_t(st_.max_utf8) + 64, 64)))) : cap_stage;
+            const size_t want = ctas(cap_in, cap_stage) + 1;
+            size_t in_b = cap_in, st_b = cap_stage;
+            while (ctas(in_b, st_b) < want && (in_b > floor_in || st_b > floor_stage)) {
+                if (in_b - floor_in >= st_b - floor_stage) in_b = std::max(floor_in, in_b - 64);
+                else st_b = std::max(floor_stage, st_b - 64);
+            }
+            if (ctas(in_b, st_b) >= want) { cap_in = in_b; cap_stage = st_b; }
+        }
         p.smem_data_cap = uint32_t(cap_in);
         p.smem_stage_cap = uint32_t(cap_stage);
         const size_t pad_smem = size_t(env_double("RV_SMEM_PAD", 0));  // development knob: occupancy sensitivity
-        smem_bytes = std::min<size_t>(smem_map(plan_nodes, S, n_slots, p.smem_data_cap, p.smem_stage_cap, use_jit).total + pad_smem, limit);
+        smem_bytes = std::min<size_t>(smem_map(plan_nodes, S, n_slots, p.smem_data_cap, p.smem_stage_cap, use_jit, item_bytes).total + pad_smem, limit);
         p.prefetch_dist = 0;
         if (!(std::getenv("RV_NO_PREFETCH") && std::getenv("RV_NO_PREFETCH")[0] == '1')) {
             // CTAs resident on the device ~ how far ahead the tile a finishing CTA's successor will take is
@@ -804,6 +822,10 @@ rv_status decode_on_device(rv_schema* s, const uint8_t* d_data, const int64_t* d
     for (int pass = 0; pass < 3; ++pass) {
         ++t_passes;
         configure(stats);
+        if (trace)
+            trace_line += "smem=" + std::to_string(smem_bytes) + "(in " + std::to_string(p.smem_data_cap) + " stage " + std::to_string(p.smem_stage_cap) +
+                          " items " + std::to_string(item_bytes) + "; largest tile seen: span " + std::to_string(stats.max_span) +
+                          " utf8 " + std::to_string(stats.max_utf8) + ") ";
         // ---- arena for this pass's capacities
         uint8_t* arena = nullptr;
         if (!count_only) {

@@ -18,6 +18,10 @@ namespace rv {
 // Source of `struct rv::gen::Walker` (includes only dev_core.cuh; also compiled for the host by tests/emu).
 std::string generate_walker_source(const Plan& plan);
 
+// Lists/maps whose items the generated walker emits item-parallel (one item per lane): those of the top-level
+// record whose items are walked.  Their item positions take item_table_bytes(n) of the CTA's shared memory.
+int item_parallel_lists(const Plan& plan);
+
 // Full NVRTC translation unit: walker + the `rvj_fused` kernel.
 std::string generate_kernel_source(const Plan& plan);
 

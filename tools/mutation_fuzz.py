@@ -3,11 +3,12 @@
 says whether the batch still decodes (then every buffer must match) or which record fails first with which category (then
 the implementation under test must say the same).
 
-    python tools/mutation_fuzz.py FIRST_SEED N [emu-interp | emu-gen | gpu-interp | gpu-jit] [--forge]
+    python tools/mutation_fuzz.py FIRST_SEED N [emu-interp | emu-gen | emu-warp | gpu-interp | gpu-jit] [--forge]
 
 --forge: structured damage instead (tests/mutation.forge_varints: edge-value / padded / over-long varints spliced in).
 
-emu-*: the host emulation of the product's readers (no GPU); gpu-*: the CUDA path through rv_decode_host.  emu-gen and
+emu-*: the host emulation of the product's readers (no GPU; emu-warp: the generated walkers with each fast emit warp in
+lock step, so the item-parallel list emit runs); gpu-*: the CUDA path through rv_decode_host.  emu-gen, emu-warp and
 gpu-jit draw their schemas from 80 seeds (one compilation each)."""
 import os
 import sys
@@ -29,6 +30,9 @@ def main():
         from tests import emu
         walker = "gen" if mode.endswith("gen") else "interp"
         decode = lambda sj, data, off, n, k: emu.decode(sj, data, off, n, k, walker=walker)  # noqa: E731
+        if mode == "emu-warp":
+            from tests.emu import warp
+            decode = warp.decode
         error_of = lambda e: (po.ERR_NAMES.get(e.code, str(e.code)), e.record) if isinstance(e, emu.EmuError) else None  # noqa: E731
         supported = lambda sj: True  # noqa: E731
     else:
@@ -36,7 +40,7 @@ def main():
         from tests.test_zz_gpu_damaged_inputs import _gpu as decode, _gpu_error as error_of
         pr.set_jit_enabled(1 if mode.endswith("jit") else 0)
         supported = lambda sj: pr.Schema(sj).is_supported  # noqa: E731
-    few = mode in ("emu-gen", "gpu-jit")
+    few = mode in ("emu-gen", "emu-warp", "gpu-jit")
     seen = {"decoded": 0, "error": 0}
     bad = 0
     t0 = time.time()
