@@ -1313,10 +1313,17 @@ class _Enc:
         self.children: List[_Enc] = []
         t = arr.type if arr is not None else None
         k = self.k
-        if k in ("int", "date"):
-            self._need(pa.types.is_int32(t) or pa.types.is_date32(t), "Int32/Date32")
-        elif k in ("long", "timestamp-millis", "timestamp-micros"):
-            self._need(pa.types.is_int64(t) or pa.types.is_timestamp(t), "Int64/Timestamp")
+        # exact downcasts, like `downcast::<Int32Array>` etc. in the reference (fast_encode.rs:196-204, 292-324)
+        if k == "int":
+            self._need(pa.types.is_int32(t), "Int32")
+        elif k == "date":
+            self._need(pa.types.is_date32(t), "Date32")
+        elif k == "long":
+            self._need(pa.types.is_int64(t), "Int64")
+        elif k == "timestamp-millis":
+            self._need(pa.types.is_timestamp(t) and t.unit == "ms", "Timestamp(ms)")
+        elif k == "timestamp-micros":
+            self._need(pa.types.is_timestamp(t) and t.unit == "us", "Timestamp(us)")
         elif k == "float":
             self._need(pa.types.is_float32(t), "Float32")
         elif k == "double":
@@ -1331,18 +1338,25 @@ class _Enc:
             for fname, fs, _ in s.fields:  # match by NAME (fast_encode.rs:157-181)
                 if fname not in names:
                     raise EncodeError(f"Arrow struct missing column '{fname}' required by Avro schema. Available columns: {names}")
-                self.children.append(_make_enc(fs, arr.field(names.index(fname)) if arr.offset == 0 else arr.field(names.index(fname))))
+                self.children.append(_make_enc(fs, arr.field(names.index(fname))))
         elif k == "union":
             self._need(pa.types.is_union(t) and t.mode == "sparse", "sparse Union")
+            if t.num_fields != len(s.variants):
+                raise EncodeError("fast_encode: union variant count mismatch")
+            # Avro variant i is the Arrow child whose type code is i (`ua.child(i as i8)`, fast_encode.rs:276)
+            codes = list(t.type_codes)
+            if sorted(codes) != list(range(len(codes))):
+                raise EncodeError(f"fast_encode: union type codes {codes} are not a permutation of 0..{len(codes) - 1}")
             for i, v in enumerate(s.variants):
-                self.children.append(_make_enc(v, arr.field(i)))
+                self.children.append(_make_enc(v, arr.field(codes.index(i))))
         elif k == "array":
             self._need(pa.types.is_list(t) and not pa.types.is_map(t), "List")
             self.children.append(_make_enc(s.items, arr.values))
         elif k == "map":
             self._need(pa.types.is_map(t), "Map")
-            self.children.append(_Enc(AvroSchema("string"), arr.keys))
-            self.children.append(_make_enc(s.values, arr.items))
+            entries = arr.values  # the raw entries struct: field() applies its own offset, which arr.keys / arr.items ignore
+            self.children.append(_Enc(AvroSchema("string"), entries.field(0)))
+            self.children.append(_make_enc(s.values, entries.field(1)))
 
     def _need(self, ok, what):
         if not ok:
@@ -1369,7 +1383,9 @@ def _np_view(buf: pa.Buffer, dtype):
 
 
 def _write(e: _Enc, row: int, out: bytearray):
-    """FieldEncoder::write (fast_encode.rs:397-502); `row` is the logical row of e.arr."""
+    """FieldEncoder::write (fast_encode.rs:397-502); `row` is the logical row of e.arr.  Struct fields and sparse
+    union children come from `field()`, which has applied the parent's offset, so they get the same logical row; list
+    and map offsets index the raw child (`arr.values`, the entries' fields) logically."""
     k = e.k
     if k == "null":
         return
@@ -1403,14 +1419,14 @@ def _write(e: _Enc, row: int, out: bytearray):
                 raise EncodeError(f"fast_encode: enum symbol '{sym}' not in schema")
             out += zigzag_bytes(e.s.symbols.index(sym))
     elif k == "record":
-        for ch in e.children:  # children of a struct share the struct's logical row (+ the struct's offset)
-            _write(ch, i, out)
+        for ch in e.children:  # field() already applied the struct's offset: children take the LOGICAL row
+            _write(ch, row, out)
     elif k == "union":
         tid = int(_np_view(bufs[0] if len(bufs) == 1 else bufs[1], "i1")[i])
         if tid < 0 or tid >= len(e.children):
             raise EncodeError(f"fast_encode: union type_id {tid} out of range")
         out += zigzag_bytes(tid)
-        _write(e.children[tid], i, out)
+        _write(e.children[tid], row, out)  # sparse: field() already applied the union's offset
     else:  # array / map (ListEncoder / MapEncoder :518-554)
         offs = _np_view(bufs[1], "<i4")
         s0, s1 = int(offs[i]), int(offs[i + 1])
@@ -1440,7 +1456,7 @@ def py_encode(schema: AvroSchema, batch: pa.RecordBatch, num_chunks: int = 1) ->
         for r in range(r0, r1):
             b = bytearray()
             for ch in top.children:
-                _write(ch, r + top.off, b)
+                _write(ch, r, b)
             rows.append(bytes(b))
         out.append(rows)
     return out

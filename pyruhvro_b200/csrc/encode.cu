@@ -404,6 +404,22 @@ struct EncBuilder {
             if (!fmt_starts(as, "+us:")) bad("fast_encode: expected (sparse) UnionArray for multi-variant union");
             if (size_t(a->n_children) != s.sub.size()) bad("fast_encode: union variant count mismatch");
             if (ulevel >= kMaxUnionLevel) bad("unions nested too deeply");
+            // Avro variant i is the Arrow child whose type code is i (`ua.child(i as i8)`, fast_encode.rs:276), so a row's
+            // type id is its Avro branch index whatever the order of the children.  Codes must be a permutation of 0..N-1.
+            std::vector<int> child_of(s.sub.size(), -1);
+            {
+                const char* f = as->format + 4;
+                bool ok = true;
+                for (size_t c = 0; c < s.sub.size() && ok; ++c) {
+                    char* e = nullptr;
+                    const long code = std::strtol(f, &e, 10);
+                    ok = e != f && (*e == ',' || (*e == '\0' && c + 1 == s.sub.size())) && code >= 0 && code < long(s.sub.size()) &&
+                         child_of[size_t(code)] < 0;
+                    if (ok) { child_of[size_t(code)] = int(c); f = *e ? e + 1 : e; }
+                }
+                if (!ok) bad(std::string("fast_encode: union type codes '") + (as->format + 4) + "' are not a permutation of 0.." +
+                             std::to_string(s.sub.size() - 1));
+            }
             const int id = new_node(NK_UNION, false, false, level, ulevel, variant);
             nodes[size_t(id)].n_variants = int32_t(s.sub.size());
             const int64_t off = base + a->offset;
@@ -411,8 +427,10 @@ struct EncBuilder {
             // sparse union: one buffer (type ids); tolerate the legacy layout with a leading null validity slot
             const void* tids = (a->n_buffers >= 2 && a->buffers[0] == nullptr) ? a->buffers[1] : a->buffers[0];
             ref_a[size_t(id)] = add_buf(tids, size_t(off + lo), size_t(off + hi));
-            for (size_t i = 0; i < s.sub.size(); ++i)
-                field(*s.sub[i], a->children[i], as->children[i], off, level + 1, ulevel + 1, int(i), depth, lo, hi);
+            for (size_t i = 0; i < s.sub.size(); ++i) {
+                const size_t c = size_t(child_of[i]);
+                field(*s.sub[i], a->children[c], as->children[c], off, level + 1, ulevel + 1, int(i), depth, lo, hi);
+            }
             nodes[size_t(id)].end = int32_t(nodes.size());
             return;
         }

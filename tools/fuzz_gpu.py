@@ -86,6 +86,11 @@ def main():
                     b = pr.deserialize_array(recs2, sj)
                     out = [bytes(x.as_py()) for a in pr.serialize_record_batch(b, sj, 3) for x in a]
                     assert out == recs2
+                    # the same rows in a layout the decoder never produces (offsets, junk, permuted union codes, ...)
+                    from tests.arrow_layouts import relayout_batch
+                    b2 = relayout_batch(b, rng)
+                    out2 = [[bytes(x.as_py()) for x in a] for a in pr.serialize_record_batch(b2, sj, 3)]
+                    assert out2 == po.py_encode(s, b2, 3) and [d for c in out2 for d in c] == recs2
             except Exception as e:
                 bad += 1
                 print(f"FAIL seed={seed} walker={walker} n={n} k={k}: {type(e).__name__}: {str(e)[:300]}\n  schema={sj[:400]}", flush=True)
