@@ -480,12 +480,15 @@ RV_HD void op_bool(C& c, bool valid, int slot_a, int slot_v, uint32_t row) {  //
 }
 
 #if defined(__CUDA_ARCH__)
-// shared -> shared copy of `len` (> 0) bytes between two shared-space addresses, one destination WORD per
-// iteration (the warp's cost is its longest string, so iterations matter).  Destination word j takes 4 source
+// shared -> shared copy of `len` (> 0) bytes between two shared-space addresses.  Destination word j takes 4 source
 // bytes at an arbitrary alignment: two aligned source words + a funnel shift.  The first and last words are
 // shared with the neighbouring strings (written by other lanes), so they are merged with an atomic OR into the
 // zero-initialised staging area; interior words are plain stores.  Source reads may touch up to 3 bytes
 // before / 4 bytes after the string: still inside the CTA's shared memory.
+// The warp's cost is its longest string, and a word-at-a-time loop makes every word wait for its own load.  So the
+// last word's loads are issued next to the first word's, and the interior words go four per trip with all of a trip's
+// loads issued together.  A string of up to 6 destination words (most real strings) then
+// waits for three rounds of loads at most.  The loop stays rolled because a generated walker has a dozen call sites.
 __device__ __forceinline__ void copy_smem_words(const uint32_t d, const uint32_t src, const uint32_t len) {
     const uint32_t a = d & 3u;
     const uint32_t nwords = (a + len + 3u) >> 2;
@@ -496,34 +499,26 @@ __device__ __forceinline__ void copy_smem_words(const uint32_t d, const uint32_t
     const uint32_t m_first = 0xFFFFFFFFu << (a * 8u);
     const uint32_t e = (a + len) & 3u;
     const uint32_t m_last = e ? (0xFFFFFFFFu >> ((4u - e) * 8u)) : 0xFFFFFFFFu;
-    uint32_t lo = lds_u32(sw), hi = lds_u32(sw + 4u);
-    uint32_t v = __funnelshift_r(lo, hi, sh);
+    const uint32_t v = __funnelshift_r(lds_u32(sw), lds_u32(sw + 4u), sh);
     if (nwords == 1u) {
         reds_or_u32(dw, v & m_first & m_last);
-    } else {
-        reds_or_u32(dw, v & m_first);
-        uint32_t j = 4;  // byte offset of the destination word being produced
-        const uint32_t last = (nwords - 1u) * 4u;
-        // (both loops are kept rolled: there are a dozen call sites per generated walker and real strings are a
-        // few words long, so unrolled copies only add code and branches — measured 5% slower)
+        return;
+    }
+    const uint32_t last = (nwords - 1u) * 4u;  // byte offset of the last destination word
+    const uint32_t vl = __funnelshift_r(lds_u32(sw + last), lds_u32(sw + last + 4u), sh);
+    reds_or_u32(dw, v & m_first);
+    reds_or_u32(dw + last, vl & m_last);
 #pragma unroll 1
-        for (; j + 16u < last; j += 16u) {  // four interior words per trip
-            const uint32_t w1 = lds_u32(sw + j + 4u), w2 = lds_u32(sw + j + 8u), w3 = lds_u32(sw + j + 12u), w4 = lds_u32(sw + j + 16u);
-            sts_u32(dw + j, __funnelshift_r(hi, w1, sh));
-            sts_u32(dw + j + 4u, __funnelshift_r(w1, w2, sh));
-            sts_u32(dw + j + 8u, __funnelshift_r(w2, w3, sh));
-            sts_u32(dw + j + 12u, __funnelshift_r(w3, w4, sh));
-            hi = w4;
-        }
-#pragma unroll 1
-        for (; j < last; j += 4u) {
-            lo = hi;
-            hi = lds_u32(sw + j + 4u);
-            sts_u32(dw + j, __funnelshift_r(lo, hi, sh));
-        }
-        lo = hi;
-        hi = lds_u32(sw + last + 4u);
-        reds_or_u32(dw + last, __funnelshift_r(lo, hi, sh) & m_last);
+    for (uint32_t j = 4u; j < last; j += 16u) {  // up to four interior words per trip
+        const uint32_t n = last - j;             // bytes of interior words from j on (>= 4)
+        const uint32_t w0 = lds_u32(sw + j), w1 = lds_u32(sw + j + 4u);
+        const uint32_t w2 = n > 4u ? lds_u32(sw + j + 8u) : 0u;
+        const uint32_t w3 = n > 8u ? lds_u32(sw + j + 12u) : 0u;
+        const uint32_t w4 = n > 12u ? lds_u32(sw + j + 16u) : 0u;
+        sts_u32(dw + j, __funnelshift_r(w0, w1, sh));
+        if (n > 4u) sts_u32(dw + j + 4u, __funnelshift_r(w1, w2, sh));
+        if (n > 8u) sts_u32(dw + j + 8u, __funnelshift_r(w2, w3, sh));
+        if (n > 12u) sts_u32(dw + j + 12u, __funnelshift_r(w3, w4, sh));
     }
 }
 #endif
