@@ -72,6 +72,19 @@ int rv_schema_is_supported(const rv_schema* s);
  * the Arrow schema ("+s" struct of the top-level fields) of the batches decode returns. */
 rv_status rv_schema_export_arrow(const rv_schema* s, struct ArrowSchema* out);
 
+/* Column projection: a new, independent handle (release it with rv_schema_release) whose batches hold only the
+ * top-level fields named in columns[0 .. n_columns), in that order.  Rows and chunking are unchanged, and every column
+ * is buffer for buffer the column of the full decode.  The other fields are still read and validated with the same
+ * checks as in a full decode, so a projected decode fails on the same record with the same status; the one exception
+ * is RV_ERR_OVERFLOW, which only a column that is produced can raise.  A selected record / list / map / union column
+ * comes out whole; nested paths ("address.city") are not supported.
+ * The handle works with every decode entry point (host, device, framed, rv_gather_*), rv_schema_export_arrow (the
+ * selected fields, same metadata), rv_schema_walker_source and rv_schema_precompile; rv_encode_host refuses it
+ * (RV_ERR_INVALID).  Projecting a projected handle selects among its columns.
+ * RV_ERR_INVALID: an empty list, a repeated name or a name that is not a top-level field (the message lists the
+ * fields).  RV_ERR_SCHEMA: `s` is not decodable. */
+rv_status rv_schema_project(const rv_schema* s, const char* const* columns, int64_t n_columns, rv_schema** out);
+
 /* ---- decode ---------------------------------------------------------------------------- */
 
 /* Replaces ruhvro::deserialize::per_datum_deserialize_threaded (ruhvro/src/deserialize.rs:76-121)
@@ -121,6 +134,11 @@ rv_status rv_decode_device_framed(const rv_schema* s, const uint8_t* d_data, con
  * runs as on any packed input.  A malformed container is RV_ERR_FRAME. */
 rv_status rv_decode_ocf_host(const uint8_t* file, int64_t len, int64_t num_chunks, rv_schema** schema_out, rv_result** out);
 
+/* rv_decode_ocf_host with a column projection (rv_schema_project) of the file's schema: *schema_out is the projected
+ * handle.  Record offsets are still found by walking every byte of every record. */
+rv_status rv_decode_ocf_host_projected(const uint8_t* file, int64_t len, int64_t num_chunks, const char* const* columns,
+                                       int64_t n_columns, rv_schema** schema_out, rv_result** out);
+
 /* Copies a device-resident result's buffers to pinned host memory (no-op if already there). */
 rv_status rv_result_to_host(rv_result* r);
 
@@ -150,6 +168,7 @@ void rv_result_free(rv_result* r);
  * reference's downcast would reject, an enum text outside the symbols or a union type id out of range are errors.
  * Rows are sliced into num_chunks chunks like slice_struct (:19-30); chunk i is exported as a Binary array
  * (i32 offsets + datum bytes), the GenericBinaryArray<i32> of the reference. */
+/* A projected handle (rv_schema_project) is RV_ERR_INVALID. */
 rv_status rv_encode_host(const rv_schema* s, struct ArrowArray* batch, struct ArrowSchema* batch_schema, int64_t num_chunks, rv_encoded** out);
 int64_t rv_encoded_num_chunks(const rv_encoded* r);
 rv_status rv_encoded_export(rv_encoded* r, int64_t chunk, struct ArrowArray* out_array, struct ArrowSchema* out_schema);

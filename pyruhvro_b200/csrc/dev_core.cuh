@@ -790,6 +790,59 @@ RV_HD bool item_stop(C& c) {
     return c.err != 0;
 }
 
+// ---- skip ops: nodes of a top-level field outside a column projection (NF_SKIP) --------------------------------
+// In either walk mode they read and check exactly what the decoding op's COUNT path reads and checks (so the FAST
+// flavour raises the same "not plain" flags and the PRECISE flavour the same first error), and store and count nothing.
+// One exception, by design: nothing of a skipped field is an Arrow offset, so it cannot overflow one (E_OVERFLOW).
+// Leaves: `kind` is a literal in the generated walkers, so the switch folds away.
+template <class C>
+RV_HD void skip_leaf(C& c, bool valid, int kind, int aux) {
+    uint32_t none = 0;  // a length summed for one value only: cannot wrap
+    switch (kind) {
+        case NK_I32: case NK_I64: op_i64<WM_COUNT, 0>(c, valid, -1, -1, 0u); break;
+        case NK_F32: op_f32<WM_COUNT, 0>(c, valid, -1, -1, 0u); break;
+        case NK_F64: op_f64<WM_COUNT, 0>(c, valid, -1, -1, 0u); break;
+        case NK_BOOL: op_bool<WM_COUNT, 0>(c, valid, -1, -1, 0u); break;
+        case NK_STR: case NK_BYTES: op_str<WM_COUNT, 0>(c, valid, -1, -1, -1, -1, 0u, none); break;
+        case NK_ENUM:  // op_enum's COUNT checks without the symbol lookup (aux = symbol count)
+            if (!valid) break;
+            if (C::kShared) {
+                if (rd_small<true>(c) >= uint32_t(aux)) c.err |= E_ENUM;
+            } else {
+                const int64_t l = rd_varint<true>(c);
+                if (!c.err && uint64_t(l) >= uint64_t(uint32_t(aux))) fail(c, E_ENUM);
+            }
+            break;
+        case NK_FIXED: op_fixed<WM_COUNT, 0>(c, valid, aux, -1, -1, 0u); break;
+        case NK_UUID: op_uuid<WM_COUNT, 0>(c, valid, -1, -1, 0u); break;
+        case NK_DEC_BYTES: op_decimal<WM_COUNT, 0>(c, valid, -1, -1, -1, 0u); break;
+        case NK_DEC_FIXED: op_decimal<WM_COUNT, 0>(c, valid, aux, -1, -1, 0u); break;
+        default: break;  // NK_NULL reads nothing
+    }
+}
+
+// Block header of a skipped list / map: rd_block's reads and checks without a row count.  0: the list ended (or an
+// error); 1: `rem` items follow; 2: read the next header (a block of zero-width items is not iterated).
+template <class C>
+RV_HD int skip_block(C& c, int64_t& rem, bool zero_items) {
+    int64_t n = rd_varint<true>(c);
+    if (C::kShared) {
+        if (n < 0 || c.err) { c.err |= E_EOF; return 0; }
+    } else {
+        if (c.err) return 0;
+        if (n < 0) {
+            (void)rd_varint<true>(c);  // block byte size: ignored, the items are always walked
+            if (c.err) return 0;
+            n = int64_t(0 - uint64_t(n));
+            if (n < 0) return 2;  // i64::MIN: an empty range
+        }
+    }
+    if (n == 0) return 0;
+    if (zero_items) return 2;
+    rem = n;
+    return 1;
+}
+
 template <int MODE, int D, class C>
 RV_HD void list_finish(C& c, bool valid, uint32_t first_row, uint32_t total, int slot_a, int slot_v, uint32_t& cur, uint32_t row) {
     if (MODE == WM_COUNT) {

@@ -47,7 +47,11 @@ enum NodeFlags : uint8_t {
     NF_NULLABLE = 1,     // wrapped in a 2-variant null union (Nullable* variants, :94-119)
     NF_NULL_FIRST = 2,   // which branch index is null (:404-414)
     NF_VALIDITY = 4,     // a validity bitmap is written for this node
-    NF_ZERO_ITEMS = 8    // list/map whose items occupy zero bytes and own no buffers
+    NF_ZERO_ITEMS = 8,   // list/map whose items occupy zero bytes and own no buffers
+    // Part of a top-level field outside a column projection: walked with the skip ops (dev_core.cuh), which read and
+    // check what the decoding op's COUNT path does and store nothing.  Such a node has no slots (-1), no stream (-1),
+    // opens no row space (space 0) and backs no OutArray; a skipped list/map keeps no row count.
+    NF_SKIP = 16
 };
 
 struct DNode {

@@ -560,6 +560,7 @@ using namespace rv;
 
 // Access to the schema internals lives in engine.cu.
 extern "C" const void* rv_schema_avro_root(const rv_schema* s);
+extern "C" int rv_schema_is_projection(const rv_schema* s);
 extern "C" void rv_set_last_error(const char* msg);
 
 struct rv_encoded {
@@ -791,6 +792,10 @@ rv_status rv_encode_host(const rv_schema* s, struct ArrowArray* batch, struct Ar
         ArrowArray* a; ArrowSchema* s;
         ~Releaser() { if (a && a->release) a->release(a); if (s && s->release) s->release(s); }
     } releaser{batch, batch_schema};
+    if (rv_schema_is_projection(s)) {
+        rv_set_last_error("fast_encode: a column projection (rv_schema_project) is not a schema to write with; encode with the full schema handle");
+        return RV_ERR_INVALID;
+    }
     if (!rv_schema_is_supported(s)) { rv_set_last_error("schema is outside the direct-encode subset; this library has no Value-tree CPU fallback"); return RV_ERR_SCHEMA; }
     const AvroNode* top = static_cast<const AvroNode*>(rv_schema_avro_root(s));
     if (std::strcmp(batch_schema->format, "+s") != 0) { rv_set_last_error("fast_encode: expected StructArray"); return RV_ERR_INVALID; }

@@ -380,11 +380,12 @@ struct SchemaStats {
 
 struct rv_schema {
     std::atomic<int> refs{1};
-    std::unique_ptr<AvroNode> avro;
+    std::shared_ptr<const AvroNode> avro;  // (shared with the handles projected from this one)
     bool supported = false;
     std::string why;              // why it is unsupported / why no plan
-    std::vector<ArrowField> fields;
+    std::vector<ArrowField> fields;  // the columns of the batches, in their order
     bool has_fields = false;
+    std::vector<int> keep;        // column projection (rv_schema_project): top-level field of each column; empty: none
     Plan plan;
     bool has_plan = false;
     std::mutex mu;
@@ -1033,6 +1034,39 @@ void rv_schema_release(rv_schema* s) {
 
 int rv_schema_is_supported(const rv_schema* s) { return s && s->supported && s->has_plan ? 1 : 0; }
 
+rv_status rv_schema_project(const rv_schema* s, const char* const* columns, int64_t n_columns, rv_schema** out) {
+    if (!s || !out || (!columns && n_columns != 0) || n_columns < 0) return fail(RV_ERR_INVALID, "null argument");
+    *out = nullptr;
+    rv_status st = check_decodable(s);
+    if (st) return st;
+    std::vector<std::string> names, requested;
+    for (const ArrowField& f : s->fields) names.push_back(f.name);
+    for (int64_t i = 0; i < n_columns; ++i) {
+        if (!columns[i]) return fail(RV_ERR_INVALID, "column projection: null column name");
+        requested.emplace_back(columns[i]);
+    }
+    try {
+        const std::vector<int> sel = select_columns(names, requested);
+        auto p = std::make_unique<rv_schema>();
+        p->avro = s->avro;
+        p->supported = true;
+        p->has_fields = true;
+        std::vector<ArrowField> all = s->keep.empty() ? s->fields : to_arrow_fields(*s->avro);
+        for (int i : sel) {
+            p->keep.push_back(s->keep.empty() ? i : s->keep[size_t(i)]);  // (a projection of a projection: fields of the schema)
+            p->fields.push_back(s->fields[size_t(i)]);
+        }
+        p->plan = build_plan(*p->avro, all, &p->keep);
+        p->has_plan = true;
+        *out = p.release();
+        return RV_OK;
+    } catch (const std::invalid_argument& e) {
+        return fail(RV_ERR_INVALID, e.what());
+    } catch (const std::exception& e) {
+        return fail(RV_ERR_SCHEMA, e.what());
+    }
+}
+
 rv_status rv_schema_export_arrow(const rv_schema* s, struct ArrowSchema* out) {
     if (!s || !out) return fail(RV_ERR_INVALID, "null argument");
     if (!s->has_fields) return fail(RV_ERR_SCHEMA, s->why.empty() ? "top-level schema is not a record" : s->why);
@@ -1423,7 +1457,11 @@ rv_status rv_ipc_close(void* p) {
 
 
 // ---- Avro object container files (ocf.hpp) ---------------------------------------------------------------------------
-extern "C" rv_status rv_decode_ocf_host(const uint8_t* file, int64_t len, int64_t num_chunks, rv_schema** schema_out, rv_result** out) {
+namespace {
+
+// rv_decode_ocf_host, and rv_decode_ocf_host_projected when `columns` is not null.
+rv_status decode_ocf(const uint8_t* file, int64_t len, int64_t num_chunks, const char* const* columns, int64_t n_columns,
+                     rv_schema** schema_out, rv_result** out) {
     if (!file || len < 0 || !schema_out || !out) return fail(RV_ERR_INVALID, "null argument");
     *schema_out = nullptr;
     *out = nullptr;
@@ -1436,6 +1474,12 @@ extern "C" rv_status rv_decode_ocf_host(const uint8_t* file, int64_t len, int64_
     rv_schema* s = nullptr;
     rv_status st = rv_schema_parse(ix.schema_json.data(), ix.schema_json.size(), &s);
     if (st) return st;
+    if (columns) {
+        rv_schema* full = s;
+        st = rv_schema_project(full, columns, n_columns, &s);
+        rv_schema_release(full);
+        if (st) return st;
+    }
     struct Release { rv_schema* s; bool armed = true; ~Release() { if (armed) rv_schema_release(s); } } rel{s};
     st = check_decodable(s);
     if (st) return st;
@@ -1492,6 +1536,19 @@ extern "C" rv_status rv_decode_ocf_host(const uint8_t* file, int64_t len, int64_
     rel.armed = false;
     *schema_out = s;
     return RV_OK;
+}
+
+}  // namespace
+
+extern "C" rv_status rv_decode_ocf_host(const uint8_t* file, int64_t len, int64_t num_chunks, rv_schema** schema_out, rv_result** out) {
+    return decode_ocf(file, len, num_chunks, nullptr, 0, schema_out, out);
+}
+
+extern "C" rv_status rv_decode_ocf_host_projected(const uint8_t* file, int64_t len, int64_t num_chunks, const char* const* columns,
+                                                  int64_t n_columns, rv_schema** schema_out, rv_result** out) {
+    if (!columns && n_columns != 0) return fail(RV_ERR_INVALID, "null argument");
+    if (!columns) return fail(RV_ERR_INVALID, "column projection: the column list is empty");
+    return decode_ocf(file, len, num_chunks, columns, n_columns, schema_out, out);
 }
 
 extern "C" {
@@ -1702,6 +1759,7 @@ rv_status rv_dev_concat_bits(uint32_t* d_dst_words, int64_t dst_bit, const uint3
 void* rv_internal_dev_get(size_t bytes, int device, size_t* actual) { return devmem().get(bytes, device, actual); }
 void rv_internal_dev_put(void* p, size_t actual, int device) { devmem().put(p, actual, device); }
 const void* rv_schema_avro_root(const rv_schema* s) { return s ? s->avro.get() : nullptr; }
+int rv_schema_is_projection(const rv_schema* s) { return s && !s->keep.empty() ? 1 : 0; }
 void rv_set_last_error(const char* msg) { t_error = msg ? msg : ""; }
 
 const char* rv_last_walker(void) { return t_walker; }

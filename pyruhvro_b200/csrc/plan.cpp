@@ -3,6 +3,7 @@
 // which Arrow buffers exist and when a validity bitmap can appear (SURVEY.md A.2).
 #include "plan.hpp"
 
+#include <algorithm>
 #include <stdexcept>
 
 namespace rv {
@@ -237,11 +238,88 @@ struct Builder {
                 throw std::runtime_error("fast_decode: unsupported schema in make_decoder: " + s.what);  // :212
         }
     }
+
+    // A field outside the column projection: the nodes build() would make, in the same pre-order, flagged NF_SKIP and
+    // owning nothing (no slots, streams, row spaces or arrays).  The same nesting limits apply: the walkers still go
+    // through every byte of it.
+    void build_skip(const AvroNode& s, const Ctx& c) {
+        const AvroNode* v = &s;
+        bool nullable = false, null_first = false;
+        if (s.k == AK::Union) {
+            if (s.sub.size() == 2 && (s.sub[0]->k == AK::Null || s.sub[1]->k == AK::Null)) {
+                null_first = s.sub[0]->k == AK::Null;
+                nullable = true;
+                v = null_first ? s.sub[1].get() : s.sub[0].get();
+                if (v->k == AK::Null || v->k == AK::Union) throw std::runtime_error("unsupported nullable inner type");
+            } else {
+                if (c.ulevel >= kMaxUnionLevel) throw std::runtime_error("unions nested deeper than " + std::to_string(kMaxUnionLevel));
+                const int id = skip_node(c, NK_UNION, false, false);
+                p.nodes[size_t(id)].aux = int32_t(s.sub.size());
+                for (size_t i = 0; i < s.sub.size(); ++i) build_skip(*s.sub[i], Ctx{c.level + 1, c.ulevel + 1, int(i), 0, c.depth, false});
+                p.nodes[size_t(id)].end = int32_t(p.nodes.size());
+                return;
+            }
+        }
+        auto leaf = [&](NodeKind nk, int aux) {
+            const int id = skip_node(c, nk, nullable, null_first);
+            p.nodes[size_t(id)].aux = aux;
+            p.nodes[size_t(id)].end = id + 1;
+        };
+        switch (v->k) {
+            case AK::Int: case AK::Date: case AK::TimeMillis: return leaf(NK_I32, 0);
+            case AK::Long: case AK::TsMillis: case AK::TsMicros: case AK::TimeMicros: return leaf(NK_I64, 0);
+            case AK::Bytes: return leaf(NK_BYTES, 0);
+            case AK::Fixed: return leaf(NK_FIXED, v->size);
+            case AK::Uuid: return leaf(NK_UUID, 16);
+            case AK::DecimalBytes: return leaf(NK_DEC_BYTES, 0);
+            case AK::DecimalFixed: return leaf(NK_DEC_FIXED, v->size);
+            case AK::Float: return leaf(NK_F32, 0);
+            case AK::Double: return leaf(NK_F64, 0);
+            case AK::Bool: return leaf(NK_BOOL, 0);
+            case AK::String: return leaf(NK_STR, 0);
+            case AK::Enum: {
+                leaf(NK_ENUM, 0);
+                p.nodes.back().aux2 = int32_t(v->symbols.size());  // the index range the walk checks
+                return;
+            }
+            case AK::Null: return leaf(NK_NULL, 0);
+            case AK::Record: {
+                if (v->fields.empty()) throw std::runtime_error("RecordDecoder produced a record with 0 fields");
+                const int id = skip_node(c, NK_REC, nullable, null_first);
+                for (auto& f : v->fields) build_skip(*f.type, Ctx{c.level + 1, c.ulevel, 0xFF, 0, c.depth, false});
+                p.nodes[size_t(id)].end = int32_t(p.nodes.size());
+                return;
+            }
+            case AK::Array: case AK::Map: {
+                const bool is_map = v->k == AK::Map;
+                if (c.depth + 1 > kMaxListDepth)
+                    throw std::runtime_error("arrays/maps nested deeper than " + std::to_string(kMaxListDepth) + " levels are not supported");
+                const int id = skip_node(c, is_map ? NK_MAP : NK_LIST, nullable, null_first);
+                const Ctx cc{c.level + 1, c.ulevel, 0xFF, 0, c.depth + 1, false};
+                if (is_map) {
+                    skip_node(cc, NK_STR, false, false);
+                    p.nodes.back().end = int32_t(p.nodes.size());
+                } else if (zero_sized(*v->sub[0])) {
+                    p.nodes[size_t(id)].flags |= NF_ZERO_ITEMS;
+                }
+                build_skip(*v->sub[0], cc);
+                p.nodes[size_t(id)].end = int32_t(p.nodes.size());
+                return;
+            }
+            default:
+                throw std::runtime_error("fast_decode: unsupported schema in make_decoder: " + v->what);
+        }
+    }
+    int skip_node(const Ctx& c, NodeKind kind, bool nullable, bool null_first) {
+        const int id = new_node(c, kind, nullable, null_first);
+        p.nodes[size_t(id)].flags |= NF_SKIP;
+        return id;
+    }
 };
 
 }  // namespace
 
-Plan build_plan(const AvroNode& top, const std::vector<ArrowField>& fields) {
+Plan build_plan(const AvroNode& top, const std::vector<ArrowField>& fields, const std::vector<int>* keep) {
     if (top.k != AK::Record) throw std::runtime_error("fast_decode::decode called on non-record schema");  // :820-823
     if (top.fields.size() != fields.size()) throw std::runtime_error("avro/arrow field count mismatch");
     // RecordBatch::try_new(schema, vec![]) at fast_decode.rs:834 (arrow-rs: a batch needs a column or a row count)
@@ -249,10 +327,15 @@ Plan build_plan(const AvroNode& top, const std::vector<ArrowField>& fields) {
     Builder b;
     b.p.space_stream.push_back(-1);
     b.p.space_depth.push_back(0);
+    std::vector<int> arr_of(top.fields.size(), -1);  // field -> its top-level array (-1: skipped)
     for (size_t i = 0; i < top.fields.size(); ++i) {
         Ctx c{1, 0, 0xFF, 0, 0, false};
-        b.p.top_arrays.push_back(b.build(*top.fields[i].type, fields[i], c));
+        const bool kept = !keep || std::find(keep->begin(), keep->end(), int(i)) != keep->end();
+        if (kept) arr_of[i] = b.build(*top.fields[i].type, fields[i], c);
+        else b.build_skip(*top.fields[i].type, c);
     }
+    if (!keep) b.p.top_arrays = arr_of;
+    else for (int f : *keep) b.p.top_arrays.push_back(arr_of.at(size_t(f)));
     return std::move(b.p);
 }
 

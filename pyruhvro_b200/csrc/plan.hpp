@@ -67,6 +67,8 @@ struct Plan {
 };
 
 // Throws std::runtime_error when the schema exceeds a documented limit.
-Plan build_plan(const AvroNode& top, const std::vector<ArrowField>& fields);
+// `keep` (a column projection, select_columns in schema.hpp): the top-level fields that become columns, in output
+// order; every other field is still walked as NF_SKIP nodes.  nullptr: every field, in schema order.
+Plan build_plan(const AvroNode& top, const std::vector<ArrowField>& fields, const std::vector<int>* keep = nullptr);
 
 }  // namespace rv

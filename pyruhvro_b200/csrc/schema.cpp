@@ -563,4 +563,21 @@ void export_arrow_schema(const std::vector<ArrowField>& fields, ArrowSchema* out
     fill_schema(top, out);
 }
 
+std::vector<int> select_columns(const std::vector<std::string>& available, const std::vector<std::string>& requested) {
+    if (requested.empty()) throw std::invalid_argument("column projection: the column list is empty");
+    std::vector<int> out;
+    std::set<std::string> seen;
+    for (const std::string& name : requested) {
+        if (!seen.insert(name).second) throw std::invalid_argument("column projection: column '" + name + "' is requested twice");
+        const auto it = std::find(available.begin(), available.end(), name);
+        if (it == available.end()) {
+            std::string avail = "[";
+            for (size_t i = 0; i < available.size(); ++i) { if (i) avail += ", "; avail += "\"" + available[i] + "\""; }
+            throw std::invalid_argument("column projection: no top-level field '" + name + "'. Available fields: " + avail + "]");
+        }
+        out.push_back(int(it - available.begin()));
+    }
+    return out;
+}
+
 }  // namespace rv

@@ -71,4 +71,9 @@ std::vector<ArrowField> to_arrow_fields(const AvroNode& top);
 // Arrow C Data Interface export of a whole schema ("+s" with the fields as children).
 void export_arrow_schema(const std::vector<ArrowField>& fields, ArrowSchema* out);
 
+// Column projection: the indices into `available` (top-level field names) of `requested`, in the requested order.
+// Throws std::invalid_argument for an empty list, a repeated name, or a name that is not a field (the message lists the
+// available ones).
+std::vector<int> select_columns(const std::vector<std::string>& available, const std::vector<std::string>& requested);
+
 }  // namespace rv

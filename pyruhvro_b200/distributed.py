@@ -69,11 +69,12 @@ def _lib():
     return lib
 
 
-def decode_sharded(schema_json: str, d_data, d_offsets, n_local: int, num_chunks: int = 1):
-    """This rank's shard -> device-resident result handle (the reference's per-chunk batches; no collective)."""
+def decode_sharded(schema_json: str, d_data, d_offsets, n_local: int, num_chunks: int = 1, *, columns=None):
+    """This rank's shard -> device-resident result handle (the reference's per-chunk batches; no collective).
+    `columns`: a column projection (top-level field names, pyruhvro_b200.Schema.project)."""
     import torch
     from . import _check, _get_or_parse_schema, lib
-    s = _get_or_parse_schema(schema_json)
+    s = _get_or_parse_schema(schema_json, columns)
     h = ctypes.c_void_p()
     _check(lib.rv_decode_device(s.handle, d_data.data_ptr(), d_offsets.data_ptr(), n_local, num_chunks,
                                 torch.cuda.current_stream().cuda_stream, ctypes.byref(h)))
@@ -165,13 +166,14 @@ def gather_result(schema, h, group=None, batch: int = 0):
         L.rv_gather_free(g)
 
 
-def decode_and_gather(schema_json: str, d_data, d_offsets, n_local: int, group=None, timing: bool = False, to_host: bool = False):
+def decode_and_gather(schema_json: str, d_data, d_offsets, n_local: int, group=None, timing: bool = False, to_host: bool = False, *,
+                      columns=None):
     """Decode this rank's shard on its GPU, then gather into single RecordBatches on the group leaders.
     Returns a dict: `batches` (pyarrow RecordBatches when to_host, else live rv_result handles freed here), timings."""
     import torch
     from . import _check, _export_batches, lib
     t0 = time.perf_counter()
-    s, h = decode_sharded(schema_json, d_data, d_offsets, n_local, 1)
+    s, h = decode_sharded(schema_json, d_data, d_offsets, n_local, 1, columns=columns)
     torch.cuda.synchronize()
     t1 = time.perf_counter()
     try:
@@ -194,7 +196,7 @@ def decode_and_gather(schema_json: str, d_data, d_offsets, n_local: int, group=N
     return out
 
 
-def decode_sharded_gather(schema_json: str, d_data, d_offsets, n_local: int, group=None) -> List[pa.RecordBatch]:
+def decode_sharded_gather(schema_json: str, d_data, d_offsets, n_local: int, group=None, *, columns=None) -> List[pa.RecordBatch]:
     """Decode + gather; the group leaders (rank 0 when everything fits one batch) get the gathered RecordBatches in
     pinned host memory, the other ranks an empty list."""
-    return decode_and_gather(schema_json, d_data, d_offsets, n_local, group=group, to_host=True)["batches"]
+    return decode_and_gather(schema_json, d_data, d_offsets, n_local, group=group, to_host=True, columns=columns)["batches"]
