@@ -70,6 +70,58 @@ def record(rng, max_items, split, first_tag=None) -> bytes:
     return bytes(out)
 
 
+def tagged(rng, tags, split=False, n_attrs=None) -> bytes:
+    """A record whose `tags` are exactly `tags` (encoded strings; None: the null branch) and with `n_attrs` map
+    entries (default: 0 to kItemSlots)."""
+    out = bytearray(varint(rng.randint(-1000, 1000)))
+    out += varint(0) if tags is None else varint(1) + blocks(tags, rng, split)
+    entries = []
+    for _ in range(rng.randint(0, K) if n_attrs is None else n_attrs):
+        entries.append(string(rng, 1, 6) + blocks([varint(rng.randint(-99, 99)) for _ in range(rng.randint(0, 3))], rng, split))
+    out += blocks(entries, rng, split)
+    out += string(rng, 0, 20)
+    return bytes(out)
+
+
+def tags_span(tags) -> int:
+    """Bytes of the list from after the union branch to after its terminating block (one block): `e = c.pos - l0`."""
+    return len(blocks(tags, None, False))
+
+
+def boundary_cases():
+    """(name, records) at the edges of the item-parallel emit.  In all but `one_lane_five` and `span_256` every lane
+    has at most kItemSlots items and its list spans at most 255 bytes."""
+    rng = random.Random(77)
+    four = [tagged(rng, [string(rng) for _ in range(K)], split=i % 2 == 1, n_attrs=K) for i in range(96)]
+    five = [record(rng, K, False) for _ in range(96)]
+    five[45] = tagged(rng, [string(rng) for _ in range(K + 1)])            # warp 1 only: kItemSeq
+    tag_255 = [varint(251) + bytes(rng.randrange(97, 123) for _ in range(251))]
+    tag_256 = [varint(252) + bytes(rng.randrange(97, 123) for _ in range(252))]
+    assert tags_span(tag_255) == 255 and tags_span(tag_256) == 256
+    span = [record(rng, K, False) for _ in range(96)]
+    span[10] = tagged(rng, tag_255)                                        # warp 0 stays item-parallel
+    span[70] = tagged(rng, tag_256)                                        # warp 2 falls back
+    empty = [record(rng, K, False) for _ in range(128)]
+    empty[32:64] = [tagged(rng, None, n_attrs=0) for _ in range(32)]       # warp 1: every lane null, no entries
+    empty[64:96] = [tagged(rng, [] if i % 2 else None, n_attrs=0) for i in range(32)]  # warp 2: null or empty
+    return [("four_each", four), ("one_lane_five", five), ("span_255_256", span), ("empty_warps", empty),
+            ("last_warp_1", [record(rng, K, True) for _ in range(97)]),
+            ("last_warp_31", [record(rng, K, True) for _ in range(127)])]
+
+
+BOUNDARY = [name for name, _ in boundary_cases()]
+
+
+@pytest.mark.parametrize("name", BOUNDARY)
+def test_item_parallel_boundaries(coracle, name):
+    """Exactly kItemSlots items in every lane (four full rounds, 128 items per warp), one lane with kItemSlots + 1, a
+    list spanning exactly 255 (item-parallel) and 256 bytes (per-lane), warps whose lanes are all null or empty (zero
+    rounds), and a last warp of 1 or 31 records."""
+    recs = dict(boundary_cases())[name]
+    for k in (1, 3):
+        check(coracle, recs, k)
+
+
 def check(coracle, recs, k=1):
     data, off = po.pack_records(recs)
     assert "items_par_" in emu.walker_source(SCHEMA)

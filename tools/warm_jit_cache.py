@@ -31,12 +31,18 @@ def schemas():
     out.append(ALL_WIDE)
     out += [gen_case_wide(seed, n=1)[0] for seed in range(30) if seed % 3]
     out.append('{"type":"record","name":"R","fields":[{"name":"id","type":"long"},{"name":"u","type":{"type":"string","logicalType":"uuid"}}]}')
+    from tests.test_gpu_fast_paths import JIT_PROJECTIONS, JIT_SCHEMAS
+    out += JIT_SCHEMAS
+    out += [(sj, tuple(cols)) for sj, cols in JIT_PROJECTIONS]  # a projected plan has its own walker
     return list(dict.fromkeys(out))
 
 
-def one(sj):
+def one(item):
+    """A schema, or (schema, columns) for a projected plan."""
     import pyruhvro_b200 as pr
-    pr.Schema(sj).precompile("sm_90a")
+    sj, cols = item if isinstance(item, tuple) else (item, None)
+    s = pr.Schema(sj)
+    (s if cols is None else s.project(list(cols))).precompile("sm_90a")
     return 1
 
 
