@@ -230,6 +230,11 @@ void rv_schema_forget_stats(const rv_schema* s);
  * with NVRTC for the device's architecture) or "interp" (the statically compiled generic kernels).
  * Both are GPU paths; RV_JIT=0 in the environment forces "interp". */
 const char* rv_last_walker(void);
+/* Records per tile (== threads per CTA) of the last decode on this thread: 256, or 384 where the generated walker
+ * decodes a plan of more than eight streams and two 384-row CTAs fit an SM (0 before any decode). */
+int rv_last_tile(void);
+/* The largest tile a decode of this schema may choose: 384 for plans of more than eight streams, else 256. */
+int rv_schema_max_tile(const rv_schema* s);
 /* Why the schema-specialised kernels are / are not in use for this schema ("ok", the NVRTC log, ...).
  * The returned string is valid until the calling thread's next library call. */
 const char* rv_schema_jit_status(const rv_schema* s);
@@ -242,9 +247,12 @@ void rv_set_jit_enabled(int enabled);
 /* The generated CUDA C++ of the schema-specialised walker (diagnostics / tests).  Returns its length;
  * copies at most cap-1 bytes + NUL into buf (buf may be NULL). */
 int64_t rv_schema_walker_source(const rv_schema* s, char* buf, size_t cap);
+/* The complete NVRTC source of the schema-specialised kernel for tiles of `tile` records (256, or
+ * rv_schema_max_tile(s)); same buffer contract.  -1 for any other tile. */
+int64_t rv_schema_kernel_source(const rv_schema* s, int tile, char* buf, size_t cap);
 
-/* Compiles the schema-specialised kernels for `arch` (e.g. "sm_90a") into the on-disk cubin cache
- * (no GPU needed), so the first decode does not pay NVRTC latency. */
+/* Compiles the schema-specialised kernel for `arch` (e.g. "sm_90a") at rv_schema_max_tile(s) into the on-disk
+ * cubin cache (no GPU needed), so the first decode does not pay NVRTC latency. */
 rv_status rv_schema_precompile(const rv_schema* s, const char* arch);
 
 const char* rv_last_error(void);

@@ -111,6 +111,11 @@ def _bind(L):
     L.rv_schema_forget_stats.argtypes = [vp]
     L.rv_schema_forget_stats.restype = None
     L.rv_last_walker.restype = cp
+    L.rv_last_tile.restype = ctypes.c_int
+    L.rv_schema_max_tile.restype = ctypes.c_int
+    L.rv_schema_max_tile.argtypes = [vp]
+    L.rv_schema_kernel_source.restype = i64
+    L.rv_schema_kernel_source.argtypes = [vp, ctypes.c_int, cp, ctypes.c_size_t]
     L.rv_set_jit_enabled.argtypes = [ctypes.c_int]
     L.rv_set_jit_enabled.restype = None
     L.rv_schema_walker_source.restype = i64

@@ -1,5 +1,6 @@
-// Kernel body of the decode: ONE fused pass per 256-record tile, templated over the walker (InterpWalker or a
-// generated, schema-specialised walker).  Device-only; compiled by nvcc (kernels.cu) and by NVRTC (jit.cpp).
+// Kernel body of the decode: ONE fused pass per kBlock-record tile (256; 384 for generated walkers of plans with more
+// than eight streams, engine.cu choose_tile), templated over the walker (InterpWalker or a generated,
+// schema-specialised walker).  Device-only; compiled by nvcc (kernels.cu) and by NVRTC (jit.cpp).
 //
 //   fused_body  one CTA per tile, tiles taken in blockIdx order:
 //     1. one TMA bulk copy (cp.async.bulk + mbarrier) stages the tile's contiguous byte window in shared memory;
@@ -184,7 +185,8 @@ __device__ __forceinline__ TileWindow stage_in(const DecodeParams& p, const Tile
     const int64_t ft = int64_t(tile_id) + p.prefetch_dist;
     if (p.prefetch_dist > 0 && ft < p.n_tiles) {
         const Tile f = tile_of(p, int(ft));
-        if (tid < 17 && f.r0 + 16 * tid <= p.n) l2_prefetch_line(p.offsets + f.r0 + 16 * tid);  // the 2 KiB (+8 B) of offsets of that tile
+        // the kBlock * 8 (+8) bytes of offsets of that tile: kBlock / 16 + 1 lines of 128 bytes
+        if (tid <= kBlock / 16 && f.r0 + 16 * tid <= p.n) l2_prefetch_line(p.offsets + f.r0 + 16 * tid);
         if (tid == kPrefetchLane) {
             w.f0 = __ldg(p.offsets + f.r0);
             w.f1 = __ldg(p.offsets + f.r0 + f.nrec);
@@ -436,10 +438,10 @@ __device__ __forceinline__ void fused_body(const DecodeParams& p, const int tile
         my_err = o.err;
     }
 
-    // ---- CTA-wide exclusive scan of every stream's lane counts.  One WARP scans one stream: each lane takes 8
-    // consecutive records (two 128-bit loads), sums them serially, and a single 5-step shuffle scan joins the 32
-    // lane totals.
-    constexpr int kPerLane = kBlock / 32;  // 4, 8, ...: a multiple of 4, so every lane moves whole uint4
+    // ---- CTA-wide exclusive scan of every stream's lane counts.  One WARP scans one stream: each lane takes kBlock / 32
+    // consecutive records (8 or 12: two or three 128-bit loads), sums them serially, and a single 5-step shuffle scan
+    // joins the 32 lane totals.  (384-row tiles give a plan of up to twelve streams one stream per warp.)
+    constexpr int kPerLane = kBlock / 32;  // 4, 8, 12, ...: a multiple of 4, so every lane moves whole uint4
     uint32_t* cur = reinterpret_cast<uint32_t*>(rv_smem + m.cur);
     uint32_t* ttot = reinterpret_cast<uint32_t*>(rv_smem + m.ttot);
     uint32_t* tbase = reinterpret_cast<uint32_t*>(rv_smem + m.tbase);

@@ -97,9 +97,14 @@ enum ErrCode : uint32_t {
 #ifndef RV_KBLOCK
 #define RV_KBLOCK 256
 #endif
-constexpr int kBlock = RV_KBLOCK;  // records per tile == threads per CTA (one record per lane)
+// Records per tile == threads per CTA (one record per lane).  The static library (interpreter, encoder) is built at
+// 256; a generated walker is compiled at its plan's tile (jit.cpp generate_kernel_source): 256, or kWideTile for
+// plans of more than kWideStreams streams, where every stream then gets a warp of its own for the scan and look-back.
+constexpr int kBlock = RV_KBLOCK;
 static_assert(kBlock % 32 == 0 && kBlock >= 64 && kBlock <= 1024, "tiles are whole warps");
 constexpr int kWarps = kBlock / 32;
+constexpr int kWideTile = 384;
+constexpr int kWideStreams = 8;
 
 // Device control block of one decode call, in 64-bit words.
 enum CtrlWord : int {
@@ -158,18 +163,19 @@ constexpr uint32_t kWindowPad = 64;
 // where the list starts in the record: the starts of its first kItemSlots items, the position after the terminating
 // block, and the item count — kItemSeq when the lane has more than kItemSlots items or the list spans more than 255
 // bytes, which makes its warp emit that list with the per-lane loop.  Entry (L, j) of lane t is byte
-// (L * kItemEntries + j) * kBlock + t.  (One byte per entry: 1.5 KiB per list keeps the Kafka plan at three CTAs per SM.)
+// (L * kItemEntries + j) * kBlock + t.  (One byte per entry: 1.5 KiB per list at 256 rows keeps the Kafka plan at three
+// CTAs per SM.)  `tile`: the tile the table is laid out for (the host sizes a generated kernel's tile, not its own kBlock).
 constexpr int kItemSlots = 4;
 constexpr int kItemEntries = kItemSlots + 2;
 constexpr uint32_t kItemSeq = 0xFFu;
 #if defined(__CUDACC__)
 __host__ __device__
 #endif
-constexpr uint32_t item_table_bytes(int n_lists) { return uint32_t(n_lists) * uint32_t(kItemEntries) * uint32_t(kBlock); }
+constexpr uint32_t item_table_bytes(int n_lists, int tile = kBlock) { return uint32_t(n_lists) * uint32_t(kItemEntries) * uint32_t(tile); }
 
 // Dynamic shared-memory map of a decode CTA (byte offsets inside the CTA's shared memory):
 //   [nodes n_nodes*32][ttot (S+1)*4][tbase S*4][adj S*4][flags 16][mbar 8][ptrs n_slots*8][items item_bytes]
-//   [cur S*kBlock*4][in: data_cap+pad][stage: stage_cap]
+//   [cur S*tile*4][in: data_cap+pad][stage: stage_cap]
 // alias_cur (walkers that keep their cursors in registers): the scan area `cur` overlays the Utf8 staging area
 // (it is dead before the first staged byte is written) and costs no extra shared memory.
 struct SmemMap {
@@ -179,7 +185,8 @@ struct SmemMap {
 #if defined(__CUDACC__)
 __host__ __device__
 #endif
-inline SmemMap smem_map(int n_nodes, int n_streams, int n_slots, uint32_t data_cap, uint32_t stage_cap, bool alias_cur, uint32_t item_bytes) {
+inline SmemMap smem_map(int n_nodes, int n_streams, int n_slots, uint32_t data_cap, uint32_t stage_cap, bool alias_cur, uint32_t item_bytes,
+                        int tile = kBlock) {
     SmemMap m;
     m.nodes = 0;
     m.ttot = uint32_t(n_nodes) * 32u;
@@ -190,7 +197,7 @@ inline SmemMap smem_map(int n_nodes, int n_streams, int n_slots, uint32_t data_c
     m.ptrs = m.mbar + 16u;
     m.items = (m.ptrs + uint32_t(n_slots) * 8u + 15u) & ~15u;
     m.cur = (m.items + item_bytes + 15u) & ~15u;
-    const uint32_t cur_bytes = uint32_t(n_streams) * kBlock * 4u;
+    const uint32_t cur_bytes = uint32_t(n_streams) * uint32_t(tile) * 4u;
     m.in = alias_cur ? m.cur : ((m.cur + cur_bytes + 15u) & ~15u);
     m.stage = (m.in + data_cap + kWindowPad + 15u) & ~15u;
     if (alias_cur) {

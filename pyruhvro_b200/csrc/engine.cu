@@ -15,6 +15,7 @@
 #include <algorithm>
 #include <atomic>
 #include <chrono>
+#include <cmath>
 #include <condition_variable>
 #include <cstdio>
 #include <cstring>
@@ -49,6 +50,7 @@ thread_local std::string t_error;
 thread_local float t_timings[6] = {0, 0, 0, 0, 0, 0};
 thread_local int t_launches = 0;
 thread_local const char* t_walker = "none";
+thread_local int t_tile = 0;  // rows per tile of the last decode (the smallest, when its chunks ran on several threads)
 thread_local long long t_slow_tiles = 0;
 thread_local int t_passes = 0;
 
@@ -376,7 +378,29 @@ struct SchemaStats {
     double in_per_row = 0;         // input bytes per record
     unsigned long long max_span = 0;   // largest tile input span (bytes)
     unsigned long long max_utf8 = 0;   // largest tile staging need (bytes)
+    int tile = 0;                      // the tile (rows) max_span and max_utf8 were measured at
 };
+
+// The largest-tile figures of `st` carried over to tiles of `tile` rows.  A tile's bytes are its rows times the mean
+// plus an excess; the excess of the largest tile is taken to grow like that of a sum of independent records (with the
+// square root of the rows).  An estimate: the first call at the new tile measures it.
+static SchemaStats stats_at(const SchemaStats& st, int tile, const Plan& plan) {
+    if (!st.valid || st.tile == tile || st.tile == 0) return st;
+    SchemaStats o = st;
+    o.tile = tile;
+    const double g = std::sqrt(double(tile) / double(st.tile));
+    auto carry = [&](unsigned long long mx, double per_row, double fixed) -> unsigned long long {
+        if (!mx) return 0;
+        const double excess = std::max(0.0, double(mx) - (per_row * st.tile + fixed));
+        return static_cast<unsigned long long>(std::ceil(per_row * tile + fixed + excess * g));
+    };
+    double utf8_per_row = 0, n_utf8 = 0;
+    for (size_t i = 0; i < plan.streams.size() && i < st.per_row.size(); ++i)
+        if (!plan.streams[i].is_rows) { utf8_per_row += st.per_row[i]; n_utf8 += 1; }
+    o.max_span = carry(st.max_span, st.in_per_row, 0.0);
+    o.max_utf8 = carry(st.max_utf8, utf8_per_row, 31.0 * n_utf8);  // (a tile's staging need has 31 bytes per column of alignment slack)
+    return o;
+}
 
 struct rv_schema {
     std::atomic<int> refs{1};
@@ -390,7 +414,7 @@ struct rv_schema {
     bool has_plan = false;
     std::mutex mu;
     std::map<int, DevicePlan> dev;  // device id -> uploaded plan
-    std::map<int, JitState> jit;    // device id -> compiled walker
+    std::map<std::pair<int, int>, JitState> jit;    // (device id, tile rows) -> compiled walker
     SchemaStats stats;
 };
 
@@ -434,15 +458,15 @@ std::string device_arch(int device) {
     return "sm_" + std::to_string(prop.major) + std::to_string(prop.minor) + ((prop.major >= 9) ? "a" : "");
 }
 
-// Compiles + loads the schema-specialised kernel once per (schema, device).  On any failure the generic
+// Compiles + loads the schema-specialised kernel once per (schema, device, tile).  On any failure the generic
 // interpreter kernel (also on the GPU) is used and the reason is kept in the state's status.
-JitState ensure_jit(rv_schema* s, int device) {
+JitState ensure_jit(rv_schema* s, int device, int tile) {
     if (!jit_enabled()) { JitState d; d.tried = true; d.status = "disabled (RV_JIT=0 / rv_set_jit_enabled(0))"; return d; }
     std::lock_guard<std::mutex> g(s->mu);
-    JitState& j = s->jit[device];
+    JitState& j = s->jit[{device, tile}];
     if (j.tried) return j;
     j.tried = true;
-    const std::string source = generate_kernel_source(s->plan), arch = device_arch(device);
+    const std::string source = generate_kernel_source(s->plan, tile), arch = device_arch(device);
     for (int attempt = 0; attempt < 2; ++attempt) {
         std::vector<char> cubin;
         std::string log;
@@ -621,9 +645,20 @@ struct SyncOnExit {
 // Hints of the host path, which can read the offsets: exact input bytes and the largest tile span.
 struct InputHints {
     int64_t total_bytes = -1;
-    int64_t max_span = -1;
+    const int64_t* offsets = nullptr;  // the call's n + 1 offsets in host memory
     rv_framing framing = {0, 0, -1};   // framed input (rv_decode_*_framed)
 };
+
+// The largest input span of a tile of `tile` rows (tiles count from each chunk's first row, as tile_of does).
+int64_t max_tile_span(const int64_t* offsets, int64_t n, int64_t k, int tile) {
+    const int64_t cr = n / k;
+    int64_t mx = 0;
+    for (int64_t j = 0; j < k; ++j) {
+        const int64_t cs = j * cr, ce = (j == k - 1) ? n : cs + cr;
+        for (int64_t a = cs; a < ce; a += tile) mx = std::max(mx, offsets[std::min(a + tile, ce)] - offsets[a]);
+    }
+    return mx;
+}
 
 // ---- the decode call ------------------------------------------------------------------------
 rv_status decode_on_device(rv_schema* s, const uint8_t* d_data, const int64_t* d_offsets, int64_t n, int64_t num_chunks,
@@ -677,17 +712,6 @@ rv_status decode_on_device(rv_schema* s, const uint8_t* d_data, const int64_t* d
     DevicePlan dp;
     rv_status st = device_plan(s, device, &dp);
     if (st) return st;
-    const int64_t tpc = std::max<int64_t>(1, (chunk_rows + kBlock - 1) / kBlock);
-    const int64_t tiles_last = (last_rows + kBlock - 1) / kBlock;
-    const int64_t n_tiles = tpc * (k - 1) + tiles_last;
-    if (n_tiles > 0x7FFFFFF0ll) return fail(RV_ERR_INVALID, "too many records for one call");
-
-    // Walker: schema-specialised (NVRTC) when available, else the generic interpreter.
-    const JitState jit = ensure_jit(s, device);
-    const bool use_jit = jit.ok;
-    t_walker = use_jit ? "jit" : "interp";
-    const int plan_nodes = use_jit ? 0 : int(plan.nodes.size());  // the generated walker has the plan baked in
-
     SchemaStats stats;
     {
         std::lock_guard<std::mutex> g(s->mu);
@@ -696,8 +720,7 @@ rv_status decode_on_device(rv_schema* s, const uint8_t* d_data, const int64_t* d
 
     DecodeParams p{};
     p.data = d_data; p.offsets = d_offsets; p.n = n; p.chunk_rows = chunk_rows; p.k = k;
-    p.tiles_per_chunk = int32_t(tpc); p.n_tiles = int32_t(n_tiles);
-    p.nodes = dp.nodes; p.n_nodes = int32_t(plan_nodes); p.n_streams = S; p.n_slots = n_slots;
+    p.n_streams = S; p.n_slots = n_slots;
     p.sym_off = dp.sym_off; p.sym_bytes = dp.sym_bytes; p.stream_slot = dp.stream_slot;
     p.n_utf8 = 0;
     for (int i = 0; i < S; ++i) p.n_utf8 += plan.streams[size_t(i)].is_rows ? 0 : 1;
@@ -705,22 +728,36 @@ rv_status decode_on_device(rv_schema* s, const uint8_t* d_data, const int64_t* d
     p.frame_check = hints.framing.check_magic ? (hints.framing.schema_id >= 0 ? 2 : 1) : 0;
     p.frame_id = uint32_t(hints.framing.schema_id >= 0 ? hints.framing.schema_id : 0);
 
-    // ---- shared-memory windows: [fixed tables][input window (+pad)][Utf8 staging / scan area] ----------
+    // ---- the walker and its tile; shared-memory windows: [fixed tables][input window (+pad)][Utf8 staging / scan area]
     const size_t limit = 227 * 1024;
-    const size_t cur_bytes = size_t(S) * kBlock * 4;
-    // the generated walker's item-position table is one of the fixed tables: it comes out of the two windows' room
-    // (configure below gives up the windows' margin where that keeps a CTA per SM)
-    const uint32_t item_bytes = use_jit ? item_table_bytes(item_parallel_lists(plan)) : 0u;
-    const size_t fixed = smem_map(plan_nodes, S, n_slots, 0, 0, use_jit, item_bytes).stage;  // everything but the two windows (incl. the pad)
-    if (fixed + (use_jit ? cur_bytes : 0) + 2048 > limit) return fail(RV_ERR_SCHEMA, "schema too wide for the shared-memory cursor table");
+    int tile = kBlock;          // rows per tile == threads per CTA
+    bool use_jit = false;       // schema-specialised walker (NVRTC), else the generic interpreter
+    int plan_nodes = 0;         // the generated walker has the plan baked in
+    uint32_t item_bytes = 0;
+    size_t cur_bytes = 0, fixed = 0;
+    int64_t span_hint = -1;     // host path: the largest tile's input span, exactly
+    auto set_walker = [&](int tile_, bool jit_) {
+        tile = tile_;
+        use_jit = jit_;
+        plan_nodes = use_jit ? 0 : int(plan.nodes.size());
+        cur_bytes = size_t(S) * size_t(tile) * 4;
+        // the generated walker's item-position table is one of the fixed tables: it comes out of the two windows' room
+        // (configure below gives up the windows' margin where that keeps a CTA per SM)
+        item_bytes = use_jit ? item_table_bytes(item_parallel_lists(plan), tile) : 0u;
+        fixed = smem_map(plan_nodes, S, n_slots, 0, 0, use_jit, item_bytes, tile).stage;  // everything but the two windows (incl. the pad)
+        span_hint = hints.offsets ? max_tile_span(hints.offsets, n, k, tile) : -1;
+    };
+    auto too_wide = [&] { return fixed + (use_jit ? cur_bytes : 0) + 2048 > limit; };
+    // CTAs of `bytes` of shared memory an SM holds; registers allow three 256-row or two 384-row CTAs (80 per thread)
+    auto ctas_per_sm = [&](size_t bytes) { const size_t c = (228 * 1024) / (bytes + 1024); return tile > kBlock ? std::min<size_t>(c, 2) : c; };
     size_t smem_bytes = 0;
     auto configure = [&](const SchemaStats& st_) {  // re-evaluated per pass: a measuring pass teaches the next one
         const double in_per_row = hints.total_bytes >= 0 ? double(hints.total_bytes) / double(n) : (st_.in_per_row > 0 ? st_.in_per_row : 128.0);
-        unsigned long long max_span = hints.max_span >= 0 ? static_cast<unsigned long long>(hints.max_span)
-                                      : (st_.max_span ? st_.max_span + st_.max_span / 16 : static_cast<unsigned long long>(in_per_row * kBlock * 1.25));
+        unsigned long long max_span = span_hint >= 0 ? static_cast<unsigned long long>(span_hint)
+                                      : (st_.max_span ? st_.max_span + st_.max_span / 16 : static_cast<unsigned long long>(in_per_row * tile * 1.25));
         // The window is sized for the LARGEST tile, so that no tile takes the slow global-memory walk; outliers beyond
         // 1.5x the mean tile are not allowed to shrink everyone's occupancy and do take it.
-        size_t want_in = std::min<size_t>(size_t(max_span), size_t(in_per_row * kBlock * env_double("RV_IN_CLAMP", 1.5))) + 48;
+        size_t want_in = std::min<size_t>(size_t(max_span), size_t(in_per_row * tile * env_double("RV_IN_CLAMP", 1.5))) + 48;
         want_in = std::max<size_t>(align_up(want_in, 64), 2048);
         const size_t room = (limit - fixed - 64) & ~size_t(15);
         const size_t min_stage = use_jit ? align_up(cur_bytes, 16) : 0;
@@ -732,7 +769,7 @@ rv_status decode_on_device(rv_schema* s, const uint8_t* d_data, const int64_t* d
             double utf8_per_row = 0;
             if (st_.valid) for (int i = 0; i < S; ++i) if (!plan.streams[size_t(i)].is_rows) utf8_per_row += st_.per_row[size_t(i)];
             size_t want_out = seen;
-            if (st_.valid) want_out = std::min<size_t>(seen, size_t(utf8_per_row * kBlock * env_double("RV_OUT_CLAMP", 1.5)) + size_t(p.n_utf8) * 31);
+            if (st_.valid) want_out = std::min<size_t>(seen, size_t(utf8_per_row * tile * env_double("RV_OUT_CLAMP", 1.5)) + size_t(p.n_utf8) * 31);
             cap_stage = align_up(want_out + 64, 64);
             if (const char* ev_ = std::getenv("RV_NO_STAGE_OUT")) if (ev_[0] == '1') cap_stage = 0;
         }
@@ -741,8 +778,8 @@ rv_status decode_on_device(rv_schema* s, const uint8_t* d_data, const int64_t* d
         // The windows carry a margin over the largest tile seen (1/16 each).  Where that margin is all that keeps the SM
         // from holding one more CTA — Kafka: windows + the item-position table just above a third of the SM — it is
         // given up, 64 bytes at a time, down to the largest tile seen; otherwise the windows stay as they are.
-        if (hints.max_span < 0 && (st_.max_span || st_.max_utf8)) {
-            auto ctas = [&](size_t in_b, size_t st_b) { return (228 * 1024) / (smem_map(plan_nodes, S, n_slots, uint32_t(in_b), uint32_t(st_b), use_jit, item_bytes).total + 1024); };
+        if (span_hint < 0 && (st_.max_span || st_.max_utf8)) {
+            auto ctas = [&](size_t in_b, size_t st_b) { return ctas_per_sm(smem_map(plan_nodes, S, n_slots, uint32_t(in_b), uint32_t(st_b), use_jit, item_bytes, tile).total); };
             const size_t floor_in = st_.max_span ? std::min(cap_in, std::max<size_t>(align_up(size_t(st_.max_span) + 48, 64), 2048)) : cap_in;
             const size_t floor_stage = st_.max_utf8 ? std::min(cap_stage, std::max(min_stage, size_t(align_up(size_t(st_.max_utf8) + 64, 64)))) : cap_stage;
             const size_t want = ctas(cap_in, cap_stage) + 1;
@@ -756,16 +793,54 @@ rv_status decode_on_device(rv_schema* s, const uint8_t* d_data, const int64_t* d
         p.smem_data_cap = uint32_t(cap_in);
         p.smem_stage_cap = uint32_t(cap_stage);
         const size_t pad_smem = size_t(env_double("RV_SMEM_PAD", 0));  // development knob: occupancy sensitivity
-        smem_bytes = std::min<size_t>(smem_map(plan_nodes, S, n_slots, p.smem_data_cap, p.smem_stage_cap, use_jit, item_bytes).total + pad_smem, limit);
+        smem_bytes = std::min<size_t>(smem_map(plan_nodes, S, n_slots, p.smem_data_cap, p.smem_stage_cap, use_jit, item_bytes, tile).total + pad_smem, limit);
         p.prefetch_dist = 0;
         if (!(std::getenv("RV_NO_PREFETCH") && std::getenv("RV_NO_PREFETCH")[0] == '1')) {
             // CTAs resident on the device ~ how far ahead the tile a finishing CTA's successor will take is
-            const int ctas_per_sm = int(std::max<size_t>(1, std::min<size_t>(8, (228 * 1024) / (smem_bytes + 1024))));
+            const int ctas = int(std::max<size_t>(1, std::min<size_t>(8, ctas_per_sm(smem_bytes))));
             int sms = 132;
             cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
-            p.prefetch_dist = sms * ctas_per_sm;
+            p.prefetch_dist = sms * ctas;
         }
     };
+    // The tile.  384 rows (kWideTile) when the walker is the generated one, the plan has more than eight streams and two
+    // 384-row CTAs fit an SM: every stream's scan and look-back then has a warp of its own (at 256 rows, eight warps
+    // take twelve streams' chains two after one another on four of them), and a third fewer tiles share the per-tile
+    // work (prologue, window staging, look-back, write-out) at the same 24 warps per SM.  Otherwise 256 rows.  Two CTAs
+    // fit when the windows as configure() sizes them for this call, the 384-row item table and scan area leave 2 x
+    // (smem + 1 KiB) within the SM's 228 KiB; __launch_bounds__(384, 2) holds the walker to 80 registers.  A call
+    // without history measures first, and its measuring pass stages no strings: it needs the input window and the
+    // scan area only.  RV_TILE=256 (development knob) keeps every plan at 256 rows for A/B runs.
+    auto choose_tile = [&]() -> JitState {
+        const char* ev_ = std::getenv("RV_TILE");
+        if (S > kWideStreams && jit_enabled() && !(ev_ && std::atoi(ev_) == kBlock)) {
+            set_walker(kWideTile, true);
+            if (!too_wide()) {
+                const SchemaStats st_ = stats_at(stats, kWideTile, plan);
+                configure(st_);
+                const size_t need = st_.valid ? smem_bytes
+                                              : smem_map(0, S, n_slots, p.smem_data_cap, uint32_t(align_up(cur_bytes, 16)), true, item_bytes, tile).total;
+                if (ctas_per_sm(need) >= 2) {
+                    const JitState j = ensure_jit(s, device, kWideTile);
+                    if (j.ok) return j;
+                }
+            }
+        }
+        const JitState j = ensure_jit(s, device, kBlock);
+        set_walker(kBlock, j.ok);
+        return j;
+    };
+    const JitState jit = choose_tile();
+    t_walker = use_jit ? "jit" : "interp";
+    t_tile = tile;
+    if (too_wide()) return fail(RV_ERR_SCHEMA, "schema too wide for the shared-memory cursor table");
+
+    const int64_t tpc = std::max<int64_t>(1, (chunk_rows + tile - 1) / tile);
+    const int64_t tiles_last = (last_rows + tile - 1) / tile;
+    const int64_t n_tiles = tpc * (k - 1) + tiles_last;
+    if (n_tiles > 0x7FFFFFF0ll) return fail(RV_ERR_INVALID, "too many records for one call");
+    p.tiles_per_chunk = int32_t(tpc); p.n_tiles = int32_t(n_tiles);
+    p.nodes = dp.nodes; p.n_nodes = int32_t(plan_nodes);
 
     // ---- per-call device state: [ctrl][bufs table][caps][null-count jobs][ones] in ONE block, initialised by one
     // copy from a pinned template and (ctrl + ones) read back by one copy ------------------------------------
@@ -822,9 +897,9 @@ rv_status decode_on_device(rv_schema* s, const uint8_t* d_data, const int64_t* d
 
     for (int pass = 0; pass < 3; ++pass) {
         ++t_passes;
-        configure(stats);
+        configure(stats_at(stats, tile, plan));
         if (trace)
-            trace_line += "smem=" + std::to_string(smem_bytes) + "(in " + std::to_string(p.smem_data_cap) + " stage " + std::to_string(p.smem_stage_cap) +
+            trace_line += "tile=" + std::to_string(tile) + " smem=" + std::to_string(smem_bytes) + "(in " + std::to_string(p.smem_data_cap) + " stage " + std::to_string(p.smem_stage_cap) +
                           " items " + std::to_string(item_bytes) + "; largest tile seen: span " + std::to_string(stats.max_span) +
                           " utf8 " + std::to_string(stats.max_utf8) + ") ";
         // ---- arena for this pass's capacities
@@ -846,8 +921,8 @@ rv_status decode_on_device(rv_schema* s, const uint8_t* d_data, const int64_t* d
         std::memset(h_misc, 0, misc_bytes);
         unsigned long long* hc = reinterpret_cast<unsigned long long*>(h_misc + off_ctrl);
         hc[CW_ERR] = ~0ull;
-        hc[CW_MAX_SPAN] = stats.max_span;   // the kernel only raises these
-        hc[CW_MAX_UTF8] = stats.max_utf8;
+        hc[CW_MAX_SPAN] = stats.tile == tile ? stats.max_span : 0ull;   // the kernel only raises these
+        hc[CW_MAX_UTF8] = stats.tile == tile ? stats.max_utf8 : 0ull;
         if (!count_only) {
             void** hb = reinterpret_cast<void**>(h_misc + off_bufs);
             for (int j = 0; j < k; ++j)
@@ -875,14 +950,14 @@ rv_status decode_on_device(rv_schema* s, const uint8_t* d_data, const int64_t* d
         RV_CUDA(cudaEventRecord(ev[0], stream));
         if (use_jit) {
             void* args[] = {&p};
-            const cudaError_t le = cudaLaunchKernel(reinterpret_cast<const void*>(jit.fused), dim3(unsigned(p.n_tiles)), dim3(kBlock), args, smem_bytes, stream);
+            const cudaError_t le = cudaLaunchKernel(reinterpret_cast<const void*>(jit.fused), dim3(unsigned(p.n_tiles)), dim3(unsigned(tile)), args, smem_bytes, stream);
             if (le != cudaSuccess) {
                 // the driver rejected the specialised kernel (attributes, architecture): remember it for this
                 // (schema, device) and decode this call with the interpreter kernel instead — still on the GPU
                 (void)cudaGetLastError();
                 {
                     std::lock_guard<std::mutex> g(s->mu);
-                    JitState& j = s->jit[device];
+                    JitState& j = s->jit[{device, tile}];
                     j.ok = false;
                     j.status = std::string("launch of the compiled walker was rejected: ") + cudaGetErrorString(le);
                 }
@@ -928,8 +1003,10 @@ rv_status decode_on_device(rv_schema* s, const uint8_t* d_data, const int64_t* d
             }
             if (hints.total_bytes >= 0) ss.in_per_row = double(hints.total_bytes) / double(n);
             else if (hb_ctrl[CW_IN_LAST] >= hb_ctrl[CW_IN_FIRST]) ss.in_per_row = double(hb_ctrl[CW_IN_LAST] - hb_ctrl[CW_IN_FIRST]) / double(n);
+            if (ss.tile != tile) ss.max_span = ss.max_utf8 = 0;  // largest tiles are per tile size: measured afresh
             ss.max_span = std::max(ss.max_span, hb_ctrl[CW_MAX_SPAN]);
             ss.max_utf8 = std::max(ss.max_utf8, hb_ctrl[CW_MAX_UTF8]);
+            ss.tile = tile;
             ss.valid = true;
             stats = ss;
         }
@@ -1205,17 +1282,7 @@ rv_status decode_host_range(rv_schema* s, const uint8_t* data, const int64_t* of
         const int64_t total = offsets[r1] - b0;
         if (total < 0) return fail(RV_ERR_INVALID, "offsets are not monotonic");
         hints.total_bytes = total;
-        // the largest tile span, exactly (the host can read the offsets): sizes the shared-memory window
-        {
-            const int64_t k = clamp_chunks(num_chunks, n);
-            const int64_t cr = n / k;
-            int64_t mx = 0;
-            for (int64_t j = 0; j < k; ++j) {
-                const int64_t cs = r0 + j * cr, ce = (j == k - 1) ? r1 : cs + cr;
-                for (int64_t a = cs; a < ce; a += kBlock) mx = std::max(mx, offsets[std::min(a + kBlock, ce)] - offsets[a]);
-            }
-            hints.max_span = mx;
-        }
+        hints.offsets = offsets + r0;  // the largest tile span, exactly (the host can read the offsets): sizes the window
         RV_CUDA(d_data.alloc(size_t(total) + 64, stream));
         RV_CUDA(d_off.alloc(size_t(n + 1) * 8, stream));
         cudaEvent_t* ev = nullptr;
@@ -1604,6 +1671,7 @@ rv_status rv_decode_host_framed(const rv_schema* s_, const uint8_t* data, const 
         int launches = 0, passes = 0;
         long long slow = 0;
         const char* walker = "none";
+        int tile = 0;
     } call;
     call.left = k;
     std::vector<rv_result*> parts(size_t(k), nullptr);
@@ -1630,6 +1698,7 @@ rv_status rv_decode_host_framed(const rv_schema* s_, const uint8_t* data, const 
             call.passes = std::max(call.passes, t_passes);
             call.slow += t_slow_tiles;
             call.walker = t_walker;
+            call.tile = call.tile ? std::min(call.tile, t_tile) : t_tile;
             if (--call.left == 0) call.cv.notify_all();
         });
     }
@@ -1642,6 +1711,7 @@ rv_status rv_decode_host_framed(const rv_schema* s_, const uint8_t* data, const 
     t_passes = call.passes;
     t_slow_tiles = call.slow;
     t_walker = call.walker;
+    t_tile = call.tile;
     auto res = std::make_unique<rv_result>();
     res->schema = rv_schema_retain(s);
     rv_status first = RV_OK;
@@ -1763,12 +1833,18 @@ int rv_schema_is_projection(const rv_schema* s) { return s && !s->keep.empty() ?
 void rv_set_last_error(const char* msg) { t_error = msg ? msg : ""; }
 
 const char* rv_last_walker(void) { return t_walker; }
+int rv_last_tile(void) { return t_tile; }
+int rv_schema_max_tile(const rv_schema* s) {
+    if (!s || !s->has_plan) return -1;
+    return int(s->plan.streams.size()) > kWideStreams ? kWideTile : kBlock;
+}
 const char* rv_schema_jit_status(const rv_schema* s) {
     if (!s) return "null schema";
     std::lock_guard<std::mutex> g(const_cast<rv_schema*>(s)->mu);
     int device = 0;
     if (cudaGetDevice(&device) != cudaSuccess) (void)cudaGetLastError();
-    auto it = s->jit.find(device);
+    auto it = s->jit.find({device, kBlock});
+    if (it == s->jit.end() || !it->second.tried) it = s->jit.find({device, kWideTile});
     t_error = (it != s->jit.end() && it->second.tried) ? it->second.status : "not attempted yet";
     return t_error.c_str();
 }
@@ -1792,12 +1868,25 @@ int64_t rv_schema_walker_source(const rv_schema* s, char* buf, size_t cap) {
     return int64_t(src.size());
 }
 
+int64_t rv_schema_kernel_source(const rv_schema* s, int tile, char* buf, size_t cap) {
+    if (!s || !s->has_plan || (tile != kBlock && tile != rv_schema_max_tile(s))) return -1;
+    const std::string src = generate_kernel_source(s->plan, tile);
+    if (buf && cap) {
+        const size_t n = std::min(cap - 1, src.size());
+        std::memcpy(buf, src.data(), n);
+        buf[n] = 0;
+    }
+    return int64_t(src.size());
+}
+
 rv_status rv_schema_precompile(const rv_schema* s, const char* arch) {
     rv_status st = check_decodable(s);
     if (st) return st;
+    // the kernel at the plan's largest tile, the one a decode takes whenever its windows allow (choose_tile); a plan of
+    // more than eight streams whose windows do not fit two 384-row CTAs compiles its 256-row kernel when first needed
     std::vector<char> cubin;
     std::string log;
-    if (!jit_cubin(generate_kernel_source(s->plan), arch && *arch ? arch : "sm_90a", &cubin, &log, false)) return fail(RV_ERR_CUDA, "NVRTC: " + log);
+    if (!jit_cubin(generate_kernel_source(s->plan, rv_schema_max_tile(s)), arch && *arch ? arch : "sm_90a", &cubin, &log, false)) return fail(RV_ERR_CUDA, "NVRTC: " + log);
     return RV_OK;
 }
 const char* rv_last_error(void) { return t_error.c_str(); }

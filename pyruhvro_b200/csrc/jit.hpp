@@ -15,15 +15,16 @@
 
 namespace rv {
 
-// Source of `struct rv::gen::Walker` (includes only dev_core.cuh; also compiled for the host by tests/emu).
-std::string generate_walker_source(const Plan& plan);
+// Source of `struct rv::gen::Walker` (includes only dev_core.cuh; also compiled for the host by tests/emu), for tiles of
+// `tile` records: the walker's item table (kItemBytes) is sized for them.
+std::string generate_walker_source(const Plan& plan, int tile = kBlock);
 
 // Lists/maps whose items the generated walker emits item-parallel (one item per lane): those of the top-level
 // record whose items are walked.  Their item positions take item_table_bytes(n) of the CTA's shared memory.
 int item_parallel_lists(const Plan& plan);
 
-// Full NVRTC translation unit: walker + the `rvj_fused` kernel.
-std::string generate_kernel_source(const Plan& plan);
+// Full NVRTC translation unit: walker + the `rvj_fused` kernel, for tiles of `tile` records (kBlock or kWideTile).
+std::string generate_kernel_source(const Plan& plan, int tile);
 
 // Compiles (or fetches from the on-disk cache) the cubin for `arch` (e.g. "sm_90a").
 // Needs no GPU.  Returns false and fills `log` when NVRTC cannot be loaded or compilation fails.

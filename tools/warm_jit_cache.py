@@ -34,6 +34,9 @@ def schemas():
     from tests.test_gpu_fast_paths import JIT_PROJECTIONS, JIT_SCHEMAS
     out += JIT_SCHEMAS
     out += [(sj, tuple(cols)) for sj, cols in JIT_PROJECTIONS]  # a projected plan has its own walker
+    from tests.test_gpu_tile384 import HB_SCHEMA, KAFKA_PROJECTIONS
+    out.append(HB_SCHEMA)
+    out += [(workloads.KAFKA_SCHEMA, tuple(cols)) for cols in KAFKA_PROJECTIONS]
     return list(dict.fromkeys(out))
 
 
