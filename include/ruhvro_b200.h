@@ -131,7 +131,11 @@ rv_status rv_decode_device_framed(const rv_schema* s, const uint8_t* d_data, con
  * uncompressed blocks only) -> `num_chunks` batches in pinned host memory.  The schema comes from the file: a new handle is
  * returned in *schema_out (release it with rv_schema_release).  Datums inside a block carry no lengths: the host walks
  * the block headers, a kernel with one lane per block walks the records to find their offsets, then the decode kernel
- * runs as on any packed input.  A malformed container is RV_ERR_FRAME. */
+ * runs as on any packed input.  A malformed container is RV_ERR_FRAME, and so is a block that claims more records than
+ * it has bytes (checked on the host, before any CUDA call): every datum takes at least one byte, so a container of a
+ * schema whose datums are always empty (records of null fields only) holds no records.  A record that fails to decode
+ * reports the error of the lowest failing record, "(record N)"; a block whose records end before its byte size is
+ * RV_ERR_FRAME at the block's last record. */
 rv_status rv_decode_ocf_host(const uint8_t* file, int64_t len, int64_t num_chunks, rv_schema** schema_out, rv_result** out);
 
 /* rv_decode_ocf_host with a column projection (rv_schema_project) of the file's schema: *schema_out is the projected

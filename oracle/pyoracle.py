@@ -650,6 +650,10 @@ def _decode(d: _Dec, c: _Cur):
                     n -= 1 << 64
             if n == 0:
                 break
+            if k == "array" and d.children[0].k == "null" and not d.children[0].nullable:
+                d.children[0].len += max(n, 0)    # items of no bytes: the loop below, without its n steps
+                d.cur += max(n, 0)
+                continue
             for _ in range(max(n, 0)):
                 if k == "map":
                     key = d.children[0]
@@ -747,6 +751,101 @@ def py_decode(schema: AvroSchema, records: List[bytes]) -> List[dict]:
             raise DecodeError(e.code, r) from None
         # trailing bytes are ignored (:825-828)
     return [_finish(d) for d in top]
+
+
+# --------------------------------------------------------------------------- #
+# Avro Object Container Files (the specification's "Object Container Files" section), uncompressed blocks only
+# --------------------------------------------------------------------------- #
+class ContainerError(ValueError):
+    """A malformed object container file: a fault of the container, not of a record."""
+
+
+OCF_MAGIC = b"Obj\x01"
+
+
+def ocf_read(file: bytes, wide: bool = False):
+    """Splits an object container file into its datums.  Returns (schema JSON text, [datum bytes], [(rec_base, count)]
+    of every block in file order, empty blocks included).
+
+    The file is the magic "Obj" 1, a header, then blocks.  The header is the file metadata, a map of bytes values
+    (written, like every Avro map, as blocks of entries: a count, negated and followed by the block's byte size when
+    negative, until a count of 0; a repeated key takes the last value), and a 16-byte sync marker.  Every block is a long
+    record count, a long byte size, that many bytes of datums and the sync marker again.  avro.schema is required;
+    avro.codec may be absent or "null" (no compression).  The datums of a block are split with this module's decoder
+    (`_Cur` / `_decode`), bounded by the block's end.
+
+    Raises ContainerError for a fault of the container, including a block that claims more records than it has bytes
+    (every datum takes at least one byte unless the schema's datums are always empty, so such a block is rejected before
+    any record is read).  Raises DecodeError(code, record) for a record fault: in each block the first record that fails,
+    at its index in the file, or "frame" at the block's last record when its datums end before its byte size; of these,
+    the lowest record wins."""
+    file = bytes(file)
+    c = _Cur(file)
+
+    def need(cond, what):
+        if not cond:
+            raise ContainerError(what)
+
+    def long_() -> int:
+        try:
+            return c.zigzag()
+        except DecodeError as e:
+            raise ContainerError(f"header varint: {e.code}") from None
+
+    def take(n: int) -> bytes:
+        need(0 <= n <= len(file) - c.p, "truncated")
+        return c.take(n)
+
+    need(file[:4] == OCF_MAGIC, "missing magic")
+    c.p = 4
+    meta = {}
+    while True:
+        n = long_()
+        if n == 0:
+            break
+        if n < 0:
+            long_()        # the block's byte size
+            n = -n
+        for _ in range(n):
+            key = take(long_())
+            meta[key] = take(long_())
+    need(b"avro.schema" in meta, "no avro.schema")
+    need(meta.get(b"avro.codec", b"null") == b"null", "compressed blocks")
+    sync = take(16)
+    schema_json = meta[b"avro.schema"].decode("utf-8")
+    spans = []             # (data start, size, count, rec_base)
+    n_records = 0
+    while c.p < len(file):
+        count, size = long_(), long_()
+        need(count >= 0 and 0 <= size <= len(file) - c.p - 16, "truncated block")
+        need(count <= size, f"block {len(spans)} holds {count} records in {size} bytes")
+        spans.append((c.p, size, count, n_records))
+        c.p += size
+        need(take(16) == sync, "sync marker mismatch")
+        n_records += count
+
+    s = parse_schema(schema_json, wide=wide)
+    if not is_supported(s):
+        raise DecodeError("schema")
+    datums, faults = [], []
+    for start, size, count, base in spans:
+        body = _Cur(file[start:start + size])
+        for i in range(count):
+            p0 = body.p
+            try:
+                for d in [_make(f[1]) for f in s.fields]:
+                    _decode(d, body)
+            except DecodeError as e:
+                faults.append((base + i, e.code))
+                break
+            datums.append(body.b[p0:body.p])
+        else:
+            if count and body.p != size:    # (the bytes of a block of no records are never read)
+                faults.append((base + count - 1, "frame"))
+    if faults:
+        record, code = min(faults)
+        raise DecodeError(code, record)
+    return schema_json, datums, [(base, count) for _, _, count, base in spans]
 
 
 def clamp_chunks(num_chunks: int, n: int) -> int:

@@ -154,6 +154,23 @@ struct DecodeParams {
     uint32_t frame_id;
 };
 
+// Object container files: where every record of every block starts (ocf.hpp, ocf_walk.cuh).
+struct OcfBlockDev { long long data_off, size, count, rec_base; };
+struct OcfParams {
+    const uint8_t* data;          // the file's bytes on the device
+    const OcfBlockDev* blocks;
+    int32_t n_blocks;
+    const DNode* nodes;
+    int32_t n_nodes;
+    int32_t n_streams;            // counters of the walk, zeroed before every record
+    const int32_t* sym_off;
+    const uint8_t* sym_bytes;
+    int64_t* offsets;             // [n_records + 1], relative to `data`
+    int64_t n_records;
+    long long end_off;
+    unsigned long long* err;      // min over (record << 8 | code); ~0 = none
+};
+
 // Readers may run a few tokens past a record's end before the deferred end-of-buffer check notices (dev_core.cuh):
 // the staged window is followed by this many readable bytes.
 constexpr uint32_t kWindowPad = 64;

@@ -1575,6 +1575,7 @@ rv_status decode_ocf(const uint8_t* file, int64_t len, int64_t num_chunks, const
         q.blocks = static_cast<const OcfBlockDev*>(d_blocks.p);
         q.n_blocks = int32_t(blocks.size());
         q.nodes = dp.nodes; q.n_nodes = int32_t(s->plan.nodes.size());
+        q.n_streams = int32_t(s->plan.streams.size());
         q.sym_off = dp.sym_off; q.sym_bytes = dp.sym_bytes;
         q.offsets = static_cast<int64_t*>(d_off.p);
         q.n_records = n;

@@ -14,6 +14,7 @@
 
 #include "dev_kernels.cuh"
 #include "interp.cuh"
+#include "ocf_walk.cuh"
 
 namespace rv {
 namespace {
@@ -57,44 +58,12 @@ __global__ void compact_kernel(const CompactJob* jobs) {
 }
 
 // ---- object container files: record offsets -------------------------------------------------------------------------
-// One LANE per block: the datums of a block carry no lengths, so the lane walks them one after the other with the
-// precise COUNT walk (full validation) straight from global memory and notes where each one starts.  Blocks are
-// independent, so a file of thousands of blocks keeps the device busy; the decode kernel then runs on the offsets like
-// on any packed input (the bytes between blocks — count, size, sync marker — trail a block's last record and are ignored
-// like any trailing bytes, fast_decode.rs:825-828).
+// One LANE per block walks the block's datums (ocf_walk.cuh).  Blocks are independent, so a file of thousands of blocks
+// keeps the device busy; the decode kernel then runs on the offsets like on any packed input.
 __global__ void ocf_offsets_kernel(const OcfParams q) {
     const int b = int(blockIdx.x * blockDim.x + threadIdx.x);
     if (b >= q.n_blocks) return;
-    const OcfBlockDev blk = q.blocks[b];
-    uint32_t cur[kMaxStreams];  // the walk's per-stream counters (unused here): local memory
-    long long pos = blk.data_off;
-    const long long end = blk.data_off + blk.size;
-    for (long long i = 0; i < blk.count; ++i) {
-        q.offsets[blk.rec_base + i] = pos;
-        WalkCtx<false> c;
-        c.nodes = q.nodes;
-        c.cur = cur;
-        c.cur_stride = 1;
-        c.sym_off = q.sym_off;
-        c.sym_bytes = q.sym_bytes;
-        c.bufs = nullptr;
-        c.ptrs_saddr = 0;
-        c.err = 0;
-        c.stage_on = false;
-        c.in_range = true;
-        c.row0 = 0;
-        c.store_word = false;
-        c.base = q.data + pos;
-        c.pos = 0;
-        const long long left = end - pos;
-        c.end = uint32_t(left > 0xFFFFFFF0ll ? 0xFFFFFFF0ll : left);
-        InterpWalker::Cur none;
-        InterpWalker::walk<WM_COUNT>(c, q.n_nodes, none);
-        if (c.err) { atomicMin(q.err, (static_cast<unsigned long long>(blk.rec_base + i) << 8) | c.err); return; }
-        pos += c.pos;
-    }
-    if (pos != end) atomicMin(q.err, (static_cast<unsigned long long>(blk.rec_base + (blk.count ? blk.count - 1 : 0)) << 8) | E_FRAME);  // the block's size disagrees with its records
-    if (b == q.n_blocks - 1) q.offsets[q.n_records] = q.end_off;
+    ocf_walk_block(q, b);
 }
 
 // ---- multi-GPU gather: every rank pushes its Arrow buffers into the gathered arena on the leader GPU ----------------

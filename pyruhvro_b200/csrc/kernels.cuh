@@ -30,22 +30,6 @@ struct PushJob {
     int32_t pad;
 };
 
-// Object container files: where every record of every block starts (ocf.hpp).
-struct OcfBlockDev { long long data_off, size, count, rec_base; };
-struct OcfParams {
-    const uint8_t* data;          // the file's bytes on the device
-    const OcfBlockDev* blocks;
-    int32_t n_blocks;
-    const DNode* nodes;
-    int32_t n_nodes;
-    const int32_t* sym_off;
-    const uint8_t* sym_bytes;
-    int64_t* offsets;             // [n_records + 1], relative to `data`
-    int64_t n_records;
-    long long end_off;
-    unsigned long long* err;      // min over (record << 8 | code); ~0 = none
-};
-
 cudaError_t prepare_kernels();  // opt in to large dynamic shared memory (once per device)
 
 void launch_fused(const DecodeParams& p, size_t smem, cudaStream_t s);   // interpreter walker, one CTA per tile

@@ -55,9 +55,14 @@ OcfIndex ocf_index(const uint8_t* file, int64_t len) {
     std::memcpy(sync, file + r.pos, 16);
     r.pos += 16;
     ix.end_off = r.pos;
-    while (r.pos < len) {
+    for (int64_t i = 0; r.pos < len; ++i) {
         const int64_t count = r.varint(), size = r.varint();
         if (count < 0 || size < 0 || size > len - r.pos - 16) r.bad("truncated block");
+        // Every datum takes at least one byte unless the schema's datums are always empty, so a block cannot hold more
+        // records than bytes.  (It also bounds the work: one lane walks `count` records and writes 8 bytes of offsets
+        // for each, so a forged count must not get that far; with it n_records <= len, and the sum cannot overflow.)
+        if (count > size)
+            r.bad(("block " + std::to_string(i) + " holds " + std::to_string(count) + " records in " + std::to_string(size) + " bytes").c_str());
         OcfBlock b{r.pos, size, count, ix.n_records};
         r.pos += size;
         if (std::memcmp(file + r.pos, sync, 16) != 0) r.bad("sync marker mismatch");

@@ -26,7 +26,8 @@ struct OcfIndex {
     int64_t end_off = 0;        // one past the last block's datums
 };
 
-// Throws std::runtime_error on a malformed container (bad magic, truncated block, sync mismatch, compressed blocks).
+// Throws std::runtime_error on a malformed container (bad magic, truncated block, sync mismatch, compressed blocks, a
+// block that claims more records than it has bytes).
 OcfIndex ocf_index(const uint8_t* file, int64_t len);
 
 }  // namespace rv

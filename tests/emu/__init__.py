@@ -9,14 +9,19 @@ import pyarrow as pa
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "..", "..", "pyruhvro_b200", "csrc")
 SO = os.path.join(HERE, "libemu.so")
-SRCS = [os.path.join(HERE, "emu.cpp")] + [os.path.join(CSRC, f) for f in ("schema.cpp", "plan.cpp", "result.cpp", "gather.cpp")]
-DEPS = SRCS + [os.path.join(CSRC, f) for f in ("dev_core.cuh", "dev_types.h", "interp.cuh", "plan.hpp", "result.hpp", "gather.hpp", "schema.hpp", "json.hpp")]
+SRCS = [os.path.join(HERE, "emu.cpp")] + [os.path.join(CSRC, f) for f in ("schema.cpp", "plan.cpp", "result.cpp", "gather.cpp", "ocf.cpp")]
+DEPS = SRCS + [os.path.join(CSRC, f) for f in ("dev_core.cuh", "dev_types.h", "interp.cuh", "ocf_walk.cuh", "plan.hpp", "result.hpp", "gather.hpp",
+                                               "ocf.hpp", "schema.hpp", "json.hpp")]
 
 
 class EmuError(ValueError):
     def __init__(self, code, record, msg=""):
         super().__init__(f"emu error {code} at record {record} {msg}")
         self.code, self.record = code, record
+
+
+class EmuContainerError(ValueError):
+    """The product's container reader (ocf.cpp) rejected an object container file."""
 
 
 def build(gen_source: str = None):
@@ -68,6 +73,31 @@ def decode(schema_json: str, data, offsets, n: int, num_chunks: int = 1, walker:
     raw = schema_json.encode()
     rc = _lib.emu_decode(raw, len(raw), data.ctypes.data if data.size else None, offsets.ctypes.data, n, num_chunks,
                          ctypes.addressof(arrs), ctypes.addressof(sch), ctypes.byref(k), ctypes.byref(rec), msg, 512)
+    if rc != 0:
+        raise EmuError(rc, rec.value, msg.value.decode())
+    schema = pa.Schema._import_from_c(ctypes.addressof(sch))
+    return [pa.RecordBatch._import_from_c(ctypes.addressof(arrs[i]), schema) for i in range(k.value)]
+
+
+def decode_ocf(file: bytes, num_chunks: int = 1):
+    """An object container file through the product's container reader, the per-block offsets walk of the device
+    (ocf_walk.cuh, every block in turn) and the emulated decode (interpreter walker).  Raises EmuContainerError for a
+    malformed container, EmuError(code, record) for a record that fails."""
+    from pyruhvro_b200 import _ArrowArray, _ArrowSchema
+    lib = _lib_interp()
+    if not hasattr(lib, "_ocf_bound"):
+        vp, i64 = ctypes.c_void_p, ctypes.c_int64
+        lib.emu_decode_ocf.argtypes = [vp, i64, i64, vp, vp, ctypes.POINTER(i64), ctypes.POINTER(i64), ctypes.c_char_p, ctypes.c_size_t]
+        lib._ocf_bound = True
+    buf = np.frombuffer(bytes(file), dtype=np.uint8)
+    arrs = (_ArrowArray * max(num_chunks, 1))()
+    sch = _ArrowSchema()
+    k, rec = ctypes.c_int64(0), ctypes.c_int64(-1)
+    msg = ctypes.create_string_buffer(512)
+    rc = lib.emu_decode_ocf(buf.ctypes.data if buf.size else None, buf.size, num_chunks, ctypes.addressof(arrs), ctypes.addressof(sch),
+                            ctypes.byref(k), ctypes.byref(rec), msg, 512)
+    if rc == -2:
+        raise EmuContainerError(msg.value.decode())
     if rc != 0:
         raise EmuError(rc, rec.value, msg.value.decode())
     schema = pa.Schema._import_from_c(ctypes.addressof(sch))

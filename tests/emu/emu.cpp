@@ -20,6 +20,8 @@
 #include "../../pyruhvro_b200/csrc/gather.hpp"
 #include "../../pyruhvro_b200/csrc/schema.hpp"
 #include "../../pyruhvro_b200/csrc/interp.cuh"
+#include "../../pyruhvro_b200/csrc/ocf.hpp"
+#include "../../pyruhvro_b200/csrc/ocf_walk.cuh"
 #ifdef EMU_GEN_WALKER
 #include EMU_GEN_WALKER   // schema-specialised walker source produced by rv_schema_walker_source()
 using EmuWalker = rv::gen::Walker;
@@ -260,6 +262,60 @@ int emu_decode(const char* json, size_t len, const uint8_t* data, const int64_t*
     try {
         Decoded d;
         const int rc = decode_core(json, len, data, off, n, num_chunks, d, err_record);
+        *k_out = d.k;
+        if (rc) return rc;
+        for (int j = 0; j < d.k; ++j) export_batch(*d.plan, d.keep->chunks[size_t(j)], d.keep->arena, d.keep, &out_batches[j]);
+        if (out_schema) export_arrow_schema(d.fields, out_schema);
+        return 0;
+    } catch (const std::exception& e) {
+        std::snprintf(msg, msg_cap, "%s", e.what());
+        return -1;
+    }
+}
+
+// ---- object container files: the product's container reader (ocf.cpp) and its per-block offsets walk (ocf_walk.cuh),
+// run for every block in turn with the kernel's error rule (lowest record << 8 | code), then the emulated decode.
+// Returns 0, a record error's code (*err_record set), -2 for a malformed container or -1 for anything else (msg set).
+int emu_decode_ocf(const uint8_t* file, int64_t len, int64_t num_chunks, ArrowArray* out_batches, ArrowSchema* out_schema,
+                   int64_t* k_out, int64_t* err_record, char* msg, size_t msg_cap) {
+    OcfIndex ix;
+    try {
+        ix = ocf_index(file, len);
+    } catch (const std::exception& e) {
+        std::snprintf(msg, msg_cap, "%s", e.what());
+        return -2;
+    }
+    try {
+        auto avro = parse_avro_schema(ix.schema_json.data(), ix.schema_json.size());
+        std::string why;
+        if (!is_supported(*avro, &why)) throw std::runtime_error("unsupported: " + why);
+        const Plan plan = build_plan(*avro, to_arrow_fields(*avro));
+        const int64_t n = ix.n_records;
+        std::vector<int64_t> off(size_t(n) + 1, ix.end_off);
+        std::vector<OcfBlockDev> blocks;
+        for (const OcfBlock& b : ix.blocks) blocks.push_back(OcfBlockDev{b.data_off, b.size, b.count, b.rec_base});
+        unsigned long long err = ~0ull;
+        OcfParams q{};
+        q.data = file;
+        q.blocks = blocks.data();
+        q.n_blocks = int32_t(blocks.size());
+        q.nodes = plan.nodes.data();
+        q.n_nodes = int32_t(plan.nodes.size());
+        q.n_streams = int32_t(plan.streams.size());
+        q.sym_off = plan.sym_off.data();
+        q.sym_bytes = plan.sym_bytes.data();
+        q.offsets = off.data();
+        q.n_records = n;
+        q.end_off = ix.end_off;
+        q.err = &err;
+        for (int b = 0; b < q.n_blocks; ++b) ocf_walk_block(q, b);
+        if (err != ~0ull) {
+            *err_record = int64_t(err >> 8);
+            *k_out = 0;
+            return int(err & 0xFF);
+        }
+        Decoded d;
+        const int rc = decode_core(ix.schema_json.data(), ix.schema_json.size(), file, off.data(), n, num_chunks, d, err_record);
         *k_out = d.k;
         if (rc) return rc;
         for (int j = 0; j < d.k; ++j) export_batch(*d.plan, d.keep->chunks[size_t(j)], d.keep->arena, d.keep, &out_batches[j]);

@@ -10,6 +10,7 @@ import pytest
 import pyruhvro_b200 as pr
 from oracle import pyoracle as po
 from tests.golden import reference_datums as G
+from tests.ocf_files import ocf_file
 from tests.parity import assert_matches_oracle, gen_case
 
 pytestmark = pytest.mark.gpu
@@ -50,48 +51,28 @@ def test_confluent_header_is_skipped_inside_the_kernel(coracle, jit):
         pr.set_jit_enabled(-1)
 
 
-def _ocf(schema_json, recs, block_records, rng, meta_extra=None):
-    def zz(v):
-        return po.zigzag_bytes(v)
-    sync = bytes(rng.randrange(256) for _ in range(16))
-    meta = {"avro.schema": schema_json.encode(), "avro.codec": b"null"}
-    meta.update(meta_extra or {})
-    out = bytearray(b"Obj\x01")
-    out += zz(len(meta))
-    for k, v in meta.items():
-        out += zz(len(k)) + k.encode() + zz(len(v)) + v
-    out += zz(0) + sync
-    i = 0
-    while i < len(recs):
-        n = min(len(recs) - i, rng.choice(block_records))
-        body = b"".join(recs[i:i + n])
-        out += zz(n) + zz(len(body)) + body + sync
-        i += n
-    return bytes(out)
-
-
 def test_object_container_file(coracle):
     import workloads
     rng = random.Random(12)
     sj, data, off = workloads.generate("kafka", 30_000, seed=4)
     recs = [data[off[i]:off[i + 1]].tobytes() for i in range(30_000)]
-    f = _ocf(sj, recs, [1, 7, 300, 1000], rng)
+    f = ocf_file(sj, recs, [1, 7, 300, 1000], rng)
     for k in (1, 4):
         got = pr.deserialize_ocf(f, k)
         assert_matches_oracle(coracle, got, sj, data, off, len(recs), k, full_validate=False)
     recs3 = [bytes.fromhex(h) for h in (G.G3_HEX, G.G4_HEX, G.G5_HEX)]      # G3 has trailing bytes inside the block: sizes disagree
     with pytest.raises(ValueError):
-        pr.deserialize_ocf(_ocf(G.G345_SCHEMA, recs3, [3], rng), 1)
+        pr.deserialize_ocf(ocf_file(G.G345_SCHEMA, recs3, [3], rng), 1)
     ok3 = [recs3[1], recs3[2]]
     d3, o3 = po.pack_records(ok3)
-    assert_matches_oracle(coracle, pr.deserialize_ocf(_ocf(G.G345_SCHEMA, ok3, [1], rng), 1), G.G345_SCHEMA, d3, o3, 2, 1)
-    assert pr.deserialize_ocf(_ocf(sj, [], [1], rng), 1)[0].num_rows == 0
+    assert_matches_oracle(coracle, pr.deserialize_ocf(ocf_file(G.G345_SCHEMA, ok3, [1], rng), 1), G.G345_SCHEMA, d3, o3, 2, 1)
+    assert pr.deserialize_ocf(ocf_file(sj, [], [1], rng), 1)[0].num_rows == 0
     with pytest.raises(ValueError, match="magic"):
         pr.deserialize_ocf(b"nope" + f[4:], 1)
     with pytest.raises(ValueError, match="sync"):
         pr.deserialize_ocf(f[:-1] + bytes([f[-1] ^ 1]), 1)
     with pytest.raises(ValueError, match="codec"):
-        pr.deserialize_ocf(_ocf(sj, recs[:10], [10], rng, {"avro.codec": b"deflate"}), 1)
-    cut = bytearray(_ocf(sj, recs[:100], [100], rng))
+        pr.deserialize_ocf(ocf_file(sj, recs[:10], [10], rng, {"avro.codec": b"deflate"}), 1)
+    cut = bytearray(ocf_file(sj, recs[:100], [100], rng))
     with pytest.raises(ValueError):
         pr.deserialize_ocf(bytes(cut[:len(cut) // 2]), 1)

@@ -234,7 +234,8 @@ def test_gpu_random_schemas(coracle, walker, n):
 @pytest.mark.gpu
 def test_gpu_every_entry_point(coracle):
     import workloads
-    from tests.test_gpu_framed import _confluent, _ocf
+    from tests.ocf_files import ocf_file
+    from tests.test_gpu_framed import _confluent
     sj, data, off = workloads.generate("kafka", 20_000, seed=5)
     n = len(off) - 1
     recs = [data[off[i]:off[i + 1]].tobytes() for i in range(n)]
@@ -247,11 +248,11 @@ def test_gpu_every_entry_point(coracle):
         _assert_selected(pr.deserialize_arrow_array(pa.array(recs, pa.binary()), sj, 3, columns=cols), want[3], cols, exp)
         _assert_selected(pr.decode_packed(data, off, n, sj, 3, columns=cols), want[3], cols, exp)
         _assert_selected(pr.deserialize_confluent(_confluent(recs, 9), sj, 3, schema_id=9, columns=cols), want[3], cols, exp)
-        _assert_selected(pr.deserialize_ocf(_ocf(sj, recs, [1, 300, 1000], random.Random(1)), 3, columns=cols), want[3], cols, exp)
+        _assert_selected(pr.deserialize_ocf(ocf_file(sj, recs, [1, 300, 1000], random.Random(1)), 3, columns=cols), want[3], cols, exp)
     with pytest.raises(ValueError, match="framed message.*record 0"):
         pr.deserialize_confluent(_confluent(recs[:10], 9), sj, 1, schema_id=8, columns=["age"])
     with pytest.raises(ValueError, match="no top-level field"):
-        pr.deserialize_ocf(_ocf(sj, recs[:10], [10], random.Random(1)), 1, columns=["nope"])
+        pr.deserialize_ocf(ocf_file(sj, recs[:10], [10], random.Random(1)), 1, columns=["nope"])
 
 
 @pytest.mark.gpu

@@ -181,12 +181,12 @@ def fuzz_ocf(first, count):
     import pyruhvro_b200 as pr
     from oracle import pyoracle as po
     from tests.parity import gen_case
-    from tests.test_gpu_framed import _ocf
+    from tests.ocf_files import ocf_file
     kinds = {}
     for seed in range(first, first + count):
         rng = random.Random(seed * 131 + 3)
         sj, recs, _, _ = gen_case(seed % 500, n=rng.choice([0, 1, 5, 40]))
-        f = bytearray(_ocf(sj, recs, [1, 3, 50], rng))
+        f = bytearray(ocf_file(sj, recs, [1, 3, 50], rng))
         for _ in range(rng.choice([1, 1, 2, 4])):
             op = rng.randrange(5)
             j = rng.randrange(len(f) + 1)

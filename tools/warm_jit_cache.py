@@ -37,6 +37,9 @@ def schemas():
     from tests.test_gpu_tile384 import HB_SCHEMA, KAFKA_PROJECTIONS
     out.append(HB_SCHEMA)
     out += [(workloads.KAFKA_SCHEMA, tuple(cols)) for cols in KAFKA_PROJECTIONS]
+    from tests.test_gpu_ocf import BIG_SCHEMA
+    from tests.test_ocf import BOOL_STR_SCHEMA, ZW_SCHEMA
+    out += [BIG_SCHEMA, BOOL_STR_SCHEMA, ZW_SCHEMA]
     return list(dict.fromkeys(out))
 
 
