@@ -85,6 +85,28 @@ rv_status rv_schema_export_arrow(const rv_schema* s, struct ArrowSchema* out);
  * fields).  RV_ERR_SCHEMA: `s` is not decodable. */
 rv_status rv_schema_project(const rv_schema* s, const char* const* columns, int64_t n_columns, rv_schema** out);
 
+/* Schema resolution (the Avro specification's "Schema Resolution", restricted as DESIGN.md §7 lists): a new, independent
+ * handle that walks datums as the WRITER's schema lays them out and returns batches in the READER's Arrow form.  A resolved
+ * decode of a datum gives the same batch, buffer for buffer, as decoding it with the writer's schema, converting the value
+ * (promotions int -> long / float / double, long -> float / double with one round-to-nearest-even step, float -> double,
+ * string <-> bytes; enum symbols by name; record fields by name or reader alias, in the reader's order; reader-only fields
+ * from their "default"; a writer non-union read as a reader ["null", T] is never null), encoding it with the reader's
+ * schema and decoding that.  Writer-only fields are read and validated as in a full decode and produce nothing.
+ * A resolved decode fails on the same record with the same status as a decode with the writer's schema, except that
+ * RV_ERR_OVERFLOW only comes from produced columns, and a writer enum symbol the reader has neither a symbol nor a
+ * default for is RV_ERR_ENUM "(record N)".
+ * The handle works with every decode entry point, rv_gather_*, rv_schema_export_arrow (exactly the reader's own
+ * schema), rv_schema_walker_source / kernel_source / max_tile / precompile and rv_schema_project (the reader's top-level
+ * fields); rv_encode_host refuses it (RV_ERR_INVALID).
+ * A reader-only field of a union type whose first branch is null may default to null whatever else the union holds
+ * (a null record, list, fixed, decimal or uuid); other defaults must be leaf values.
+ * RV_ERR_SCHEMA, naming the reader field's path ("address.country"): a pair outside the rules, a reader-only field
+ * without a default or with one that does not match its type or is a record / list / map / fixed / decimal / uuid
+ * value, unions with branches added, removed or reordered, a
+ * writer union read as a non-union, promotions between logical types.  RV_ERR_INVALID: a projected or resolved handle
+ * passed as writer or reader. */
+rv_status rv_schema_resolve(const rv_schema* writer, const rv_schema* reader, rv_schema** out);
+
 /* ---- decode ---------------------------------------------------------------------------- */
 
 /* Replaces ruhvro::deserialize::per_datum_deserialize_threaded (ruhvro/src/deserialize.rs:76-121)
@@ -142,6 +164,11 @@ rv_status rv_decode_ocf_host(const uint8_t* file, int64_t len, int64_t num_chunk
  * handle.  Record offsets are still found by walking every byte of every record. */
 rv_status rv_decode_ocf_host_projected(const uint8_t* file, int64_t len, int64_t num_chunks, const char* const* columns,
                                        int64_t n_columns, rv_schema** schema_out, rv_result** out);
+/* The file's records read with `reader` (rv_schema_resolve: the file's schema is the writer's), optionally projected to
+ * the reader's top-level fields columns[0 .. n_columns) (columns may be NULL with n_columns 0).  The record offsets are
+ * still found by walking the writer's schema.  *schema_out is the resolved (and projected) handle. */
+rv_status rv_decode_ocf_host_resolved(const uint8_t* file, int64_t len, int64_t num_chunks, const rv_schema* reader,
+                                      const char* const* columns, int64_t n_columns, rv_schema** schema_out, rv_result** out);
 
 /* Copies a device-resident result's buffers to pinned host memory (no-op if already there). */
 rv_status rv_result_to_host(rv_result* r);

@@ -81,6 +81,8 @@ def _bind(L):
     L.rv_decode_ocf_host.argtypes = [vp, i64, i64, ctypes.POINTER(vp), ctypes.POINTER(vp)]
     L.rv_decode_ocf_host_projected.argtypes = [vp, i64, i64, vp, i64, ctypes.POINTER(vp), ctypes.POINTER(vp)]
     L.rv_schema_project.argtypes = [vp, vp, i64, ctypes.POINTER(vp)]
+    L.rv_schema_resolve.argtypes = [vp, vp, ctypes.POINTER(vp)]
+    L.rv_decode_ocf_host_resolved.argtypes = [vp, i64, i64, vp, vp, i64, ctypes.POINTER(vp), ctypes.POINTER(vp)]
     L.rv_result_to_host.argtypes = [vp]
     L.rv_result_num_batches.restype = i64
     L.rv_result_num_batches.argtypes = [vp]
@@ -176,6 +178,15 @@ class Schema:
         _check(lib.rv_schema_project(self.handle, names, len(keep), ctypes.byref(h)))
         return Schema._adopt(h.value)
 
+    def read_as(self, reader_json: str) -> "Schema":
+        """A schema that reads data written with this schema (the writer's) as `reader_json` (rv_schema_resolve): batches
+        in the reader's Arrow form, fields matched by name or reader alias, reader-only fields filled from their defaults,
+        promotions and enum symbols resolved per the Avro specification."""
+        reader = reader_json if isinstance(reader_json, Schema) else _get_or_parse_schema(reader_json)
+        h = ctypes.c_void_p()
+        _check(lib.rv_schema_resolve(self.handle, reader.handle, ctypes.byref(h)))
+        return Schema._adopt(h.value)
+
     @property
     def is_supported(self) -> bool:
         return bool(lib.rv_schema_is_supported(self.handle))
@@ -215,24 +226,32 @@ def _column_names(columns):
     return arr, keep
 
 
-# schema_cache / get_or_parse_schema (src/lib.rs:39-54): unbounded, keyed by the exact string and the column projection
+# schema_cache / get_or_parse_schema (src/lib.rs:39-54): unbounded, keyed by the exact strings of the (writer) schema and
+# the reader schema, and the column projection
 _schema_cache = {}
 _schema_lock = threading.Lock()
 
 
-def _get_or_parse_schema(schema: str, columns=None) -> Schema:
+def _get_or_parse_schema(schema: str, columns=None, reader_schema=None) -> Schema:
     if not isinstance(schema, str):
         raise TypeError("argument 'schema': expected str")
+    if reader_schema is not None and not isinstance(reader_schema, str):
+        raise TypeError("argument 'reader_schema': expected str")
     if columns is not None:
         if isinstance(columns, (str, bytes)):
             raise TypeError("argument 'columns': expected a list of field names, not a single string")
         columns = tuple(columns)
-    key = (schema, columns)
+    key = (schema, reader_schema, columns)
     with _schema_lock:
         s = _schema_cache.get(key)
     if s is not None:
         return s
-    parsed = Schema(schema) if columns is None else _get_or_parse_schema(schema).project(columns)
+    if columns is not None:
+        parsed = _get_or_parse_schema(schema, None, reader_schema).project(columns)
+    elif reader_schema is not None:
+        parsed = _get_or_parse_schema(schema).read_as(reader_schema)
+    else:
+        parsed = Schema(schema)
     with _schema_lock:
         return _schema_cache.setdefault(key, parsed)
 
@@ -268,10 +287,10 @@ class Framing(ctypes.Structure):
     _fields_ = [("header_bytes", ctypes.c_int32), ("check_magic", ctypes.c_int32), ("schema_id", ctypes.c_int64)]
 
 
-def _decode_list(records, schema: str, num_chunks: int, framing=None, columns=None) -> List[pa.RecordBatch]:
+def _decode_list(records, schema: str, num_chunks: int, framing=None, columns=None, reader_schema=None) -> List[pa.RecordBatch]:
     if not isinstance(records, list):
         raise TypeError("argument 'list': expected a list of bytes")
-    s = _get_or_parse_schema(schema, columns)
+    s = _get_or_parse_schema(schema, columns, reader_schema)
     if framing is None:
         handle = _ext().decode_list(s.handle, records, int(num_chunks))
     else:
@@ -281,17 +300,25 @@ def _decode_list(records, schema: str, num_chunks: int, framing=None, columns=No
 
 # Every decode entry point takes a keyword-only `columns`: a list of top-level field names.  The batches then hold only
 # those columns, in that order, each identical to that column of the full decode (Schema.project).
+# And a keyword-only `reader_schema`: the schema to read the data as (Schema.read_as); `schema` stays the schema the data
+# was written with.  With both, `columns` names the reader's fields.
 
 
-def deserialize_ocf(data, num_chunks=1, *, columns=None) -> List[pa.RecordBatch]:
+def deserialize_ocf(data, num_chunks=1, *, columns=None, reader_schema=None) -> List[pa.RecordBatch]:
     """The bytes of an Avro Object Container File (uncompressed blocks) -> `num_chunks` RecordBatches; the schema is the
-    file's own.  Record boundaries are found on the GPU (one lane per block), see include/ruhvro_b200.h."""
+    file's own (with `reader_schema`: the file's schema is the writer's, the batches are the reader's).  Record boundaries
+    are found on the GPU (one lane per block), see include/ruhvro_b200.h."""
     import numpy as np
     if num_chunks < 0:
         raise OverflowError("can't convert negative int to unsigned")
     buf = np.frombuffer(data, dtype=np.uint8)
     sh, h = ctypes.c_void_p(), ctypes.c_void_p()
-    if columns is None:
+    if reader_schema is not None:
+        reader = _get_or_parse_schema(reader_schema)
+        names, keep = _column_names(columns) if columns is not None else (None, [])
+        _check(lib.rv_decode_ocf_host_resolved(buf.ctypes.data if buf.size else None, buf.size, int(num_chunks), reader.handle,
+                                               names, len(keep), ctypes.byref(sh), ctypes.byref(h)))
+    elif columns is None:
         _check(lib.rv_decode_ocf_host(buf.ctypes.data if buf.size else None, buf.size, int(num_chunks), ctypes.byref(sh), ctypes.byref(h)))
     else:
         names, keep = _column_names(columns)
@@ -300,40 +327,41 @@ def deserialize_ocf(data, num_chunks=1, *, columns=None) -> List[pa.RecordBatch]
     return _export_batches(h.value, Schema._adopt(sh.value))
 
 
-def deserialize_confluent(list, schema, num_chunks=1, schema_id=None, *, columns=None):  # noqa: A002
+def deserialize_confluent(list, schema, num_chunks=1, schema_id=None, *, columns=None, reader_schema=None):  # noqa: A002
     """list[bytes] of Confluent-framed Kafka messages (magic 0x00 + big-endian u32 schema id + Avro datum) ->
     `num_chunks` RecordBatches.  The 5-byte header is validated (the id too when `schema_id` is given) and skipped inside
     the decode kernel — no per-message slicing in Python (the reference expects callers to strip it, README.md:93-94)."""
     if num_chunks < 0:
         raise OverflowError("can't convert negative int to unsigned")
-    return _decode_list(list, schema, num_chunks, framing=(5, 1, -1 if schema_id is None else int(schema_id)), columns=columns)
+    return _decode_list(list, schema, num_chunks, framing=(5, 1, -1 if schema_id is None else int(schema_id)), columns=columns,
+                        reader_schema=reader_schema)
 
 
-def deserialize_array(list, schema, *, columns=None):  # noqa: A002 - the reference names the parameter `list`
+def deserialize_array(list, schema, *, columns=None, reader_schema=None):  # noqa: A002 - the reference names the parameter `list`
     """list[bytes] of schemaless Avro datums -> one RecordBatch (src/lib.rs:56-71)."""
-    return _decode_list(list, schema, 1, columns=columns)[0]
+    return _decode_list(list, schema, 1, columns=columns, reader_schema=reader_schema)[0]
 
 
-def deserialize_array_threaded(list, schema, num_chunks, *, columns=None):  # noqa: A002
+def deserialize_array_threaded(list, schema, num_chunks, *, columns=None, reader_schema=None):  # noqa: A002
     """list[bytes] -> `num_chunks` RecordBatches over contiguous row ranges (src/lib.rs:73-89;
     chunking per ruhvro/src/deserialize.rs:53-68)."""
     if num_chunks < 0:
         raise OverflowError("can't convert negative int to unsigned")  # usize extraction in PyO3
-    return _decode_list(list, schema, num_chunks, columns=columns)
+    return _decode_list(list, schema, num_chunks, columns=columns, reader_schema=reader_schema)
 
 
-def deserialize_array_threaded_spawn(list, schema, num_chunks, *, columns=None):  # noqa: A002
+def deserialize_array_threaded_spawn(list, schema, num_chunks, *, columns=None, reader_schema=None):  # noqa: A002
     """Same results as deserialize_array_threaded (the reference only changes the tokio primitive,
     ruhvro/src/deserialize.rs:123-170)."""
-    return deserialize_array_threaded(list, schema, num_chunks, columns=columns)
+    return deserialize_array_threaded(list, schema, num_chunks, columns=columns, reader_schema=reader_schema)
 
 
 def decode_packed(data, offsets, n: int, schema: str, num_chunks: int = 1, framing: "Framing | None" = None, *,
-                  columns=None) -> List[pa.RecordBatch]:
+                  columns=None, reader_schema=None) -> List[pa.RecordBatch]:
     """Packed host buffers (numpy uint8 data + int64 offsets[n+1]) -> batches, through rv_decode_host (or
     rv_decode_host_framed when `framing` is given).  This is the C-ABI call a Rust/FFI caller makes; no Python list walk."""
     import numpy as np
-    s = _get_or_parse_schema(schema, columns)
+    s = _get_or_parse_schema(schema, columns, reader_schema)
     data = np.ascontiguousarray(data, dtype=np.uint8)
     offsets = np.ascontiguousarray(offsets, dtype=np.int64)
     h = ctypes.c_void_p()
@@ -366,7 +394,7 @@ def _packed_view(arr):
     return data, off.astype(np.int64, copy=False), n
 
 
-def deserialize_arrow_array(array, schema, num_chunks=1, *, columns=None):
+def deserialize_arrow_array(array, schema, num_chunks=1, *, columns=None, reader_schema=None):
     """An Arrow Binary/LargeBinary array (or ChunkedArray) of schemaless datums -> `num_chunks` RecordBatches.
 
     The ingest shortcut of SURVEY §8(f) rank 2: what `per_datum_deserialize_threaded` builds internally at
@@ -375,7 +403,7 @@ def deserialize_arrow_array(array, schema, num_chunks=1, *, columns=None):
     if num_chunks < 0:
         raise OverflowError("can't convert negative int to unsigned")
     data, off, n = _packed_view(array)
-    return decode_packed(data, off, n, schema, int(num_chunks), columns=columns)
+    return decode_packed(data, off, n, schema, int(num_chunks), columns=columns, reader_schema=reader_schema)
 
 
 def serialize_record_batch(data, schema, num_chunks):

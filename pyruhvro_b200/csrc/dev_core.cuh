@@ -590,12 +590,16 @@ RV_HD void op_str(C& c, bool valid, int slot_a, int slot_b, int slot_v, int stre
 }
 
 template <int MODE, int D, class C>
-RV_HD void op_enum(C& c, bool valid, int slot_a, int slot_b, int slot_v, int stream, uint32_t row, int sym_base, int n_sym, uint32_t& cur) {  // append_enum :570-578
+// `remap` (NF_ENUM_MAP, resolved plans): a writer symbol whose entry after the table's n + 1 offsets is non-zero has no
+// reader symbol, and its record fails with E_ENUM_MAP.
+RV_HD void op_enum(C& c, bool valid, int slot_a, int slot_b, int slot_v, int stream, uint32_t row, int sym_base, int n_sym, uint32_t& cur,
+                   bool remap = false) {  // append_enum :570-578
     uint32_t len = 0;
     if (valid) {
         if (C::kShared) {  // FAST
             uint32_t l = rd_small<MODE == WM_COUNT>(c);
             if (MODE == WM_COUNT && l >= uint32_t(n_sym)) { c.err |= E_ENUM; l = 0; }
+            if (MODE == WM_COUNT && remap && c.sym_off[sym_base + n_sym + 1 + int32_t(l)]) c.err |= E_ENUM_MAP;
             const int32_t b0 = c.sym_off[sym_base + int32_t(l)];
             len = uint32_t(c.sym_off[sym_base + int32_t(l) + 1] - b0);
             if (MODE == WM_EMIT) copy_from_symbols(c, slot_b, stream, cur, c.sym_bytes + b0, len);
@@ -603,6 +607,7 @@ RV_HD void op_enum(C& c, bool valid, int slot_a, int slot_b, int slot_v, int str
             const int64_t l = rd_varint<MODE == WM_COUNT>(c);
             if (MODE == WM_COUNT && c.err) valid = false;
             else if (MODE == WM_COUNT && uint64_t(l) >= uint64_t(uint32_t(n_sym))) { fail(c, E_ENUM); valid = false; }
+            else if (MODE == WM_COUNT && remap && c.sym_off[sym_base + n_sym + 1 + int32_t(l)]) { fail(c, E_ENUM_MAP); valid = false; }
             else {
                 const int32_t b0 = c.sym_off[sym_base + int32_t(l)];
                 len = uint32_t(c.sym_off[sym_base + int32_t(l) + 1] - b0);
@@ -611,6 +616,96 @@ RV_HD void op_enum(C& c, bool valid, int slot_a, int slot_b, int slot_v, int str
         }
     }
     utf8_finish<MODE, D>(c, valid, len, slot_a, slot_v, cur, row);
+}
+
+// ---- schema resolution (rv_schema_resolve) ----------------------------------------------------------------------
+// Bit patterns of a converted value.  One rounding step, to nearest even (__ll2float_rn / __ll2double_rn; on the host the
+// default rounding mode of the conversion does the same).
+RV_HD uint32_t f32_bits_of_i64(int64_t v) {
+#if defined(__CUDA_ARCH__)
+    return __float_as_uint(__ll2float_rn(v));
+#else
+    const float f = float(v);
+    uint32_t u;
+    __builtin_memcpy(&u, &f, 4);
+    return u;
+#endif
+}
+RV_HD uint64_t f64_bits_of_i64(int64_t v) {
+#if defined(__CUDA_ARCH__)
+    return uint64_t(__double_as_longlong(__ll2double_rn(v)));
+#else
+    const double d = double(v);
+    uint64_t u;
+    __builtin_memcpy(&u, &d, 8);
+    return u;
+#endif
+}
+RV_HD uint64_t f64_bits_of_f32(uint32_t w) {  // exact
+#if defined(__CUDA_ARCH__)
+    return uint64_t(__double_as_longlong(double(__uint_as_float(w))));
+#else
+    float f;
+    __builtin_memcpy(&f, &w, 4);
+    const double d = f;
+    uint64_t u;
+    __builtin_memcpy(&u, &d, 8);
+    return u;
+#endif
+}
+
+// NK_PROMOTE: the writer's value as op_i32 / op_i64 / op_f32 read it (with their checks), stored as the reader's type.
+template <int MODE, int D, class C>
+RV_HD void op_promote(C& c, bool valid, int from, int to, int slot_a, int slot_v, uint32_t row) {
+    uint64_t bits = 0;
+    if (valid) {
+        if (from == NK_F32) {
+            if (!C::kShared && MODE == WM_COUNT && c.end - c.pos < 4u) { fail(c, E_EOF); valid = false; }
+            else {
+                if (MODE == WM_EMIT) bits = f64_bits_of_f32(ld_le32(c, c.pos));
+                c.pos += 4;
+            }
+        } else {
+            const int64_t x = rd_varint<MODE == WM_COUNT>(c);
+            if (C::kShared || MODE == WM_EMIT || !c.err) {
+                const int64_t v = from == NK_I32 ? int64_t(int32_t(x)) : x;  // an int is the `as i32` of its varint
+                if (MODE == WM_EMIT) bits = to == NK_I64 ? uint64_t(v) : (to == NK_F32 ? uint64_t(f32_bits_of_i64(v)) : f64_bits_of_i64(v));
+            } else {
+                valid = false;
+            }
+        }
+    }
+    if (MODE == WM_EMIT) {
+        if (may_store<D>(c)) {
+            if (to == NK_F32) static_cast<uint32_t*>(buf_ptr(c, slot_a))[row] = uint32_t(bits);
+            else static_cast<uint64_t*>(buf_ptr(c, slot_a))[row] = bits;
+        }
+        if (slot_v >= 0) put_bit<D>(c, slot_v, row, valid);
+    }
+}
+
+// NK_DEFAULT: reads nothing.  `valid` is false where the parent is absent.  A Utf8 default counts its bytes into the
+// node's stream like any string and copies them from the symbol table.
+template <int MODE, int D, class C>
+RV_HD void op_default(C& c, bool valid, int out, int lo, int hi, int slot_a, int slot_b, int slot_v, int stream, uint32_t row, uint32_t& cur) {
+    if (out == NK_STR) {
+        uint32_t len = 0;
+        if (valid) {
+            const int32_t b0 = c.sym_off[lo];
+            len = uint32_t(c.sym_off[lo + 1] - b0);
+            if (MODE == WM_EMIT && len) copy_from_symbols(c, slot_b, stream, cur, c.sym_bytes + b0, len);
+        }
+        utf8_finish<MODE, D>(c, valid, len, slot_a, slot_v, cur, row);
+        return;
+    }
+    if (MODE != WM_EMIT) return;
+    if (out == NK_BOOL) {
+        put_bit<D>(c, slot_a, row, valid && lo != 0);
+    } else if (may_store<D>(c)) {
+        if (out == NK_I32 || out == NK_F32) static_cast<uint32_t*>(buf_ptr(c, slot_a))[row] = valid ? uint32_t(lo) : 0u;
+        else static_cast<uint64_t*>(buf_ptr(c, slot_a))[row] = valid ? ((uint64_t(uint32_t(hi)) << 32) | uint32_t(lo)) : 0ull;
+    }
+    if (slot_v >= 0) put_bit<D>(c, slot_v, row, valid);
 }
 
 // ---- the wider subset (SURVEY.md 8(f) rank 3): bytes, fixed, uuid, decimal -------------------------------------

@@ -359,7 +359,8 @@ __device__ __forceinline__ void emit_walk(const DecodeParams& p, const Tile& t, 
             for (int i = tid & 31; i < p.n_nodes; i += 32) {  // (every warp: a warp may be alone on the precise path)
                 const DNode nd = c.nodes[i];
                 if (nd.flags & NF_SKIP) continue;  // owns no buffers
-                if (nd.kind == NK_STR || nd.kind == NK_ENUM || nd.kind == NK_LIST || nd.kind == NK_MAP || nd.kind == NK_BYTES)
+                if (nd.kind == NK_STR || nd.kind == NK_ENUM || nd.kind == NK_LIST || nd.kind == NK_MAP || nd.kind == NK_BYTES ||
+                    (nd.kind == NK_DEFAULT && nd.pad0 == NK_STR))
                     static_cast<int32_t*>(buf_ptr(c, nd.slot_a))[0] = 0;
             }
         } else {

@@ -40,7 +40,14 @@ enum NodeKind : uint8_t {
     NK_FIXED = 13,     // fixed(N) -> FixedSizeBinary(N): N raw bytes, aux = N
     NK_DEC_BYTES = 14, // decimal on bytes -> Decimal128: varint length + big-endian two's complement
     NK_DEC_FIXED = 15, // decimal on fixed(N) -> Decimal128: N big-endian bytes, aux = N
-    NK_UUID = 16       // uuid (string logical type) -> FixedSizeBinary(16): 36-char hyphenated hex text
+    NK_UUID = 16,      // uuid (string logical type) -> FixedSizeBinary(16): 36-char hyphenated hex text
+    // schema resolution (rv_schema_resolve)
+    NK_PROMOTE = 17,   // a writer int / long / float read as a reader long / float / double: aux = writer kind (NK_I32, NK_I64,
+                       // NK_F32), aux2 = reader kind (NK_I64, NK_F32, NK_F64)
+    NK_DEFAULT = 18    // a reader field the writer does not have: reads nothing, writes its (non-null) default on every row.
+                       // pad0 = the column's kind (NK_I32, NK_I64, NK_F32, NK_F64, NK_BOOL; NK_STR for string / bytes / enum
+                       // text); aux / aux2 = the low / high 32 bits of the value, or (NK_STR) aux = the first of the two
+                       // symbol-table entries that bound its bytes.  (A null default is an NF_ABSENT subtree.)
 };
 
 enum NodeFlags : uint8_t {
@@ -51,7 +58,15 @@ enum NodeFlags : uint8_t {
     // Part of a top-level field outside a column projection: walked with the skip ops (dev_core.cuh), which read and
     // check what the decoding op's COUNT path does and store nothing.  Such a node has no slots (-1), no stream (-1),
     // opens no row space (space 0) and backs no OutArray; a skipped list/map keeps no row count.
-    NF_SKIP = 16
+    NF_SKIP = 16,
+    // NK_ENUM of a resolved plan whose writer has symbols the reader cannot map: the symbol table holds, after the n + 1
+    // offsets, n words that are non-zero for those symbols.  A record that has one fails with E_ENUM_MAP.
+    NF_ENUM_MAP = 32,
+    // The root of a subtree that is never present: a reader-only field of a nullable type whose default is null (resolved
+    // plans).  The walkers treat it like a node whose parent is absent -- the append_null path of every op, reading
+    // nothing -- so its buffers are those of a null of the reader's own type: a cleared validity bit, zeroed values, an
+    // unchanged offset, type id 0, and the same for every descendant.
+    NF_ABSENT = 64
 };
 
 struct DNode {
@@ -91,6 +106,7 @@ enum ErrCode : uint32_t {
     E_SCHEMA = 7,
     E_OVERFLOW = 8,  // i32 Arrow offset overflow (arrow-rs panics; reported as an error)
     E_FRAME = 12,    // framed input (SURVEY.md 8(f) rank 4): message shorter than its header / wrong magic byte / wrong schema id
+    E_ENUM_MAP = 13, // resolved plans: a writer enum symbol with neither a reader symbol nor a reader default (reported as RV_ERR_ENUM)
     E_VALUE = 11     // wider subset: a value its logical type cannot hold (uuid text that is not a UUID, decimal wider than 128 bits)
 };
 

@@ -793,7 +793,7 @@ rv_status rv_encode_host(const rv_schema* s, struct ArrowArray* batch, struct Ar
         ~Releaser() { if (a && a->release) a->release(a); if (s && s->release) s->release(s); }
     } releaser{batch, batch_schema};
     if (rv_schema_is_projection(s)) {
-        rv_set_last_error("fast_encode: a column projection (rv_schema_project) is not a schema to write with; encode with the full schema handle");
+        rv_set_last_error("fast_encode: a column projection (rv_schema_project) or a resolved handle (rv_schema_resolve) is not a schema to write with; encode with the full schema handle");
         return RV_ERR_INVALID;
     }
     if (!rv_schema_is_supported(s)) { rv_set_last_error("schema is outside the direct-encode subset; this library has no Value-tree CPU fallback"); return RV_ERR_SCHEMA; }

@@ -410,6 +410,9 @@ struct rv_schema {
     std::vector<ArrowField> fields;  // the columns of the batches, in their order
     bool has_fields = false;
     std::vector<int> keep;        // column projection (rv_schema_project): top-level field of each column; empty: none
+    // schema resolution (rv_schema_resolve): `avro` is the writer's schema, `reader` the reader's, `res` pairs them
+    std::shared_ptr<const AvroNode> reader;
+    std::shared_ptr<const Resolution> res;
     Plan plan;
     bool has_plan = false;
     std::mutex mu;
@@ -523,6 +526,9 @@ struct rv_result {
 
 namespace {
 
+// The status of a record's error code (E_ENUM_MAP is an RV_ERR_ENUM with a message of its own).
+rv_status status_of(uint32_t code) { return code == E_ENUM_MAP ? RV_ERR_ENUM : rv_status(code); }
+
 const char* err_text(uint32_t code) {
     switch (code) {
         case E_EOF: return "unexpected end of buffer";
@@ -531,6 +537,7 @@ const char* err_text(uint32_t code) {
         case E_NEG_LEN: return "negative string length";
         case E_BRANCH: return "invalid union branch index";
         case E_ENUM: return "enum index out of range";
+        case E_ENUM_MAP: return "enum symbol has neither a reader symbol nor a reader default";
         case E_OVERFLOW: return "Arrow i32 offset overflow (or malformed input offsets)";
         case E_VALUE: return "value does not fit its logical type (uuid text / decimal wider than 128 bits)";
         case E_FRAME: return "framed message: shorter than its header, wrong magic byte or unexpected schema id";
@@ -883,7 +890,8 @@ rv_status decode_on_device(rv_schema* s, const uint8_t* d_data, const int64_t* d
             for (int i = 0; i < S; ++i) {
                 double want = double(rows_of(j)) * stats.per_row[size_t(i)] * margin + 4096.0;
                 const Stream& st_ = plan.streams[size_t(i)];
-                const bool enum_text = !st_.is_rows && plan.nodes[size_t(st_.node)].kind == NK_ENUM;  // symbol text is not input bytes
+                const bool enum_text = !st_.is_rows && (plan.nodes[size_t(st_.node)].kind == NK_ENUM ||
+                                                        plan.nodes[size_t(st_.node)].kind == NK_DEFAULT);  // symbol / default text is not input bytes
                 if (!enum_text) want = std::min(want, in_bytes + 4096.0);
                 caps[size_t(j) * size_t(Sx) + size_t(i)] = static_cast<unsigned long long>(std::min(want, 2147483647.0));
                 planned += want;
@@ -983,7 +991,7 @@ rv_status decode_on_device(rv_schema* s, const uint8_t* d_data, const int64_t* d
         const unsigned long long err_word = hb_ctrl[CW_ERR];
         if (err_word != ~0ull) {
             const uint32_t code = uint32_t(err_word & 0xFF);
-            return fail(rv_status(code), std::string(err_text(code)) + " (record " + std::to_string(int64_t(err_word >> 8) + record_base) + ")");
+            return fail(status_of(code), std::string(err_text(code)) + " (record " + std::to_string(int64_t(err_word >> 8) + record_base) + ")");
         }
         std::memcpy(chunk_tot.data(), hb_ctrl + CW_CHUNK_TOT, chunk_tot.size() * 8);
         const bool over = hb_ctrl[CW_OVER] != 0ull;
@@ -1128,17 +1136,46 @@ rv_status rv_schema_project(const rv_schema* s, const char* const* columns, int6
         p->avro = s->avro;
         p->supported = true;
         p->has_fields = true;
-        std::vector<ArrowField> all = s->keep.empty() ? s->fields : to_arrow_fields(*s->avro);
+        p->reader = s->reader;
+        p->res = s->res;
+        const AvroNode& out_schema = s->res ? *s->reader : *s->avro;  // (a resolved handle's columns are the reader's fields)
+        std::vector<ArrowField> all = s->keep.empty() ? s->fields : to_arrow_fields(out_schema);
         for (int i : sel) {
             p->keep.push_back(s->keep.empty() ? i : s->keep[size_t(i)]);  // (a projection of a projection: fields of the schema)
             p->fields.push_back(s->fields[size_t(i)]);
         }
-        p->plan = build_plan(*p->avro, all, &p->keep);
+        p->plan = p->res ? build_resolved_plan(*p->res, all, &p->keep) : build_plan(*p->avro, all, &p->keep);
         p->has_plan = true;
         *out = p.release();
         return RV_OK;
     } catch (const std::invalid_argument& e) {
         return fail(RV_ERR_INVALID, e.what());
+    } catch (const std::exception& e) {
+        return fail(RV_ERR_SCHEMA, e.what());
+    }
+}
+
+rv_status rv_schema_resolve(const rv_schema* writer, const rv_schema* reader, rv_schema** out) {
+    if (!writer || !reader || !out) return fail(RV_ERR_INVALID, "null argument");
+    *out = nullptr;
+    if (!writer->keep.empty() || writer->res || !reader->keep.empty() || reader->res)
+        return fail(RV_ERR_INVALID, "schema resolution: pass the handles of the writer's and the reader's full schemas (rv_schema_parse)");
+    rv_status st = check_decodable(writer);
+    if (st) return st;
+    st = check_decodable(reader);
+    if (st) return st;
+    try {
+        auto p = std::make_unique<rv_schema>();
+        p->avro = writer->avro;
+        p->reader = reader->avro;
+        p->res = std::make_shared<const Resolution>(resolve_schemas(*p->avro, *p->reader));
+        p->supported = true;
+        p->fields = reader->fields;
+        p->has_fields = true;
+        p->plan = build_resolved_plan(*p->res, p->fields);
+        p->has_plan = true;
+        *out = p.release();
+        return RV_OK;
     } catch (const std::exception& e) {
         return fail(RV_ERR_SCHEMA, e.what());
     }
@@ -1526,9 +1563,10 @@ rv_status rv_ipc_close(void* p) {
 // ---- Avro object container files (ocf.hpp) ---------------------------------------------------------------------------
 namespace {
 
-// rv_decode_ocf_host, and rv_decode_ocf_host_projected when `columns` is not null.
+// rv_decode_ocf_host, rv_decode_ocf_host_projected when `columns` is not null, rv_decode_ocf_host_resolved when `reader` is
+// not null.
 rv_status decode_ocf(const uint8_t* file, int64_t len, int64_t num_chunks, const char* const* columns, int64_t n_columns,
-                     rv_schema** schema_out, rv_result** out) {
+                     rv_schema** schema_out, rv_result** out, const rv_schema* reader = nullptr) {
     if (!file || len < 0 || !schema_out || !out) return fail(RV_ERR_INVALID, "null argument");
     *schema_out = nullptr;
     *out = nullptr;
@@ -1541,6 +1579,13 @@ rv_status decode_ocf(const uint8_t* file, int64_t len, int64_t num_chunks, const
     rv_schema* s = nullptr;
     rv_status st = rv_schema_parse(ix.schema_json.data(), ix.schema_json.size(), &s);
     if (st) return st;
+    rv_schema* file_schema = nullptr;  // resolved: the record offsets are found by walking the file's (the writer's) own plan
+    if (reader) {
+        st = rv_schema_resolve(s, reader, &file_schema);
+        std::swap(s, file_schema);
+        if (st) { rv_schema_release(file_schema); return st; }
+    }
+    struct ReleaseFile { rv_schema* s; ~ReleaseFile() { if (s) rv_schema_release(s); } } rel_file{file_schema};
     if (columns) {
         rv_schema* full = s;
         st = rv_schema_project(full, columns, n_columns, &s);
@@ -1562,8 +1607,9 @@ rv_status decode_ocf(const uint8_t* file, int64_t len, int64_t num_chunks, const
     SyncOnExit guard{stream};
     RV_CUDA(upload(static_cast<uint8_t*>(d_file.p), file, size_t(len), device, stream));
     if (n > 0) {
+        rv_schema* walk_schema = file_schema ? file_schema : s;
         DevicePlan dp;
-        st = device_plan(s, device, &dp);
+        st = device_plan(walk_schema, device, &dp);
         if (st) return st;
         std::vector<OcfBlockDev> blocks(ix.blocks.size());
         for (size_t i = 0; i < blocks.size(); ++i) blocks[i] = OcfBlockDev{ix.blocks[i].data_off, ix.blocks[i].size, ix.blocks[i].count, ix.blocks[i].rec_base};
@@ -1574,8 +1620,8 @@ rv_status decode_ocf(const uint8_t* file, int64_t len, int64_t num_chunks, const
         q.data = static_cast<const uint8_t*>(d_file.p);
         q.blocks = static_cast<const OcfBlockDev*>(d_blocks.p);
         q.n_blocks = int32_t(blocks.size());
-        q.nodes = dp.nodes; q.n_nodes = int32_t(s->plan.nodes.size());
-        q.n_streams = int32_t(s->plan.streams.size());
+        q.nodes = dp.nodes; q.n_nodes = int32_t(walk_schema->plan.nodes.size());
+        q.n_streams = int32_t(walk_schema->plan.streams.size());
         q.sym_off = dp.sym_off; q.sym_bytes = dp.sym_bytes;
         q.offsets = static_cast<int64_t*>(d_off.p);
         q.n_records = n;
@@ -1588,7 +1634,7 @@ rv_status decode_ocf(const uint8_t* file, int64_t len, int64_t num_chunks, const
         RV_CUDA(cudaStreamSynchronize(stream));   // (the block table on the host stack is done with as well)
         if (err_word != ~0ull) {
             const uint32_t code = uint32_t(err_word & 0xFF);
-            return fail(rv_status(code), std::string(err_text(code)) + " (record " + std::to_string(int64_t(err_word >> 8)) + ")");
+            return fail(status_of(code), std::string(err_text(code)) + " (record " + std::to_string(int64_t(err_word >> 8)) + ")");
         }
     }
     try {
@@ -1617,6 +1663,12 @@ extern "C" rv_status rv_decode_ocf_host_projected(const uint8_t* file, int64_t l
     if (!columns && n_columns != 0) return fail(RV_ERR_INVALID, "null argument");
     if (!columns) return fail(RV_ERR_INVALID, "column projection: the column list is empty");
     return decode_ocf(file, len, num_chunks, columns, n_columns, schema_out, out);
+}
+
+extern "C" rv_status rv_decode_ocf_host_resolved(const uint8_t* file, int64_t len, int64_t num_chunks, const rv_schema* reader,
+                                                 const char* const* columns, int64_t n_columns, rv_schema** schema_out, rv_result** out) {
+    if (!reader || (!columns && n_columns != 0)) return fail(RV_ERR_INVALID, "null argument");
+    return decode_ocf(file, len, num_chunks, columns, n_columns, schema_out, out, reader);
 }
 
 extern "C" {
@@ -1830,7 +1882,7 @@ rv_status rv_dev_concat_bits(uint32_t* d_dst_words, int64_t dst_bit, const uint3
 void* rv_internal_dev_get(size_t bytes, int device, size_t* actual) { return devmem().get(bytes, device, actual); }
 void rv_internal_dev_put(void* p, size_t actual, int device) { devmem().put(p, actual, device); }
 const void* rv_schema_avro_root(const rv_schema* s) { return s ? s->avro.get() : nullptr; }
-int rv_schema_is_projection(const rv_schema* s) { return s && !s->keep.empty() ? 1 : 0; }
+int rv_schema_is_projection(const rv_schema* s) { return s && (!s->keep.empty() || s->res) ? 1 : 0; }  // (or a resolution)
 void rv_set_last_error(const char* msg) { t_error = msg ? msg : ""; }
 
 const char* rv_last_walker(void) { return t_walker; }

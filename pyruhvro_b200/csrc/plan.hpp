@@ -71,4 +71,11 @@ struct Plan {
 // order; every other field is still walked as NF_SKIP nodes.  nullptr: every field, in schema order.
 Plan build_plan(const AvroNode& top, const std::vector<ArrowField>& fields, const std::vector<int>* keep = nullptr);
 
+// A resolved plan (rv_schema_resolve): the walk follows the writer's schema as `res` (resolve_schemas) pairs it with the
+// reader's, and the output tree is the reader's, in the reader's field order at every depth (`fields`: the reader's
+// to_arrow_fields).  Writer-only fields become NF_SKIP subtrees, reader-only fields NK_DEFAULT leaves placed after their
+// record's writer fields, promotions NK_PROMOTE leaves.  `keep`: the reader's top-level fields that become columns, in
+// output order (nullptr: all); the writer fields behind the others are skipped.
+Plan build_resolved_plan(const Resolution& res, const std::vector<ArrowField>& fields, const std::vector<int>* keep = nullptr);
+
 }  // namespace rv

@@ -2,6 +2,9 @@
 #include "schema.hpp"
 
 #include <algorithm>
+#include <cerrno>
+#include <climits>
+#include <cstdint>
 #include <cstdlib>
 #include <cstring>
 #include <map>
@@ -30,9 +33,10 @@ std::unique_ptr<AvroNode> clone_node(const AvroNode& n) {
     auto c = std::make_unique<AvroNode>();
     c->k = n.k; c->fullname = n.fullname; c->has_doc = n.has_doc; c->doc = n.doc; c->has_aliases = n.has_aliases;
     c->aliases = n.aliases; c->symbols = n.symbols; c->what = n.what; c->size = n.size; c->precision = n.precision; c->scale = n.scale;
+    c->has_enum_default = n.has_enum_default; c->enum_default = n.enum_default;
     for (auto& f : n.fields) {
         AvroField cf;
-        cf.name = f.name; cf.has_doc = f.has_doc; cf.doc = f.doc;
+        cf.name = f.name; cf.has_doc = f.has_doc; cf.doc = f.doc; cf.dflt = f.dflt; cf.aliases = f.aliases;
         cf.type = clone_node(*f.type);
         c->fields.push_back(std::move(cf));
     }
@@ -239,6 +243,10 @@ std::unique_ptr<AvroNode> parse_node(const Json& j, const std::string& ns, int d
             else if (ft->is_string() && ft->str == "fixed") f.type = parse_node(fj, rns, depth + 1, names);  // {"name":..,"type":"fixed","size":..}: the field object is the fixed
             else f.type = parse_node(*ft, rns, depth + 1, names);
             if (const Json* d = fj.find("doc"); d && d->is_string()) { f.has_doc = true; f.doc = d->str; }
+            if (const Json* d = fj.find("default")) f.dflt = std::make_shared<const Json>(*d);   // (checked when a resolution uses it)
+            if (const Json* a = fj.find("aliases"); a && a->kind == Json::Array)
+                for (auto& al : a->arr)
+                    if (al.is_string()) f.aliases.push_back(al.str);
             r->fields.push_back(std::move(f));
         }
         names.open.erase(r->fullname);
@@ -262,6 +270,8 @@ std::unique_ptr<AvroNode> parse_node(const Json& j, const std::string& ns, int d
         if (const Json* d = j.find("default")) {   // Error::EnumDefaultWrongType / Error::GetEnumDefault
             if (!d->is_string()) bad("enum default must be a string");
             if (std::find(e->symbols.begin(), e->symbols.end(), d->str) == e->symbols.end()) bad("enum default \"" + d->str + "\" is not one of the symbols");
+            e->has_enum_default = true;
+            e->enum_default = d->str;
         }
         names.done[e->fullname] = e.get();
         return e;
@@ -578,6 +588,250 @@ std::vector<int> select_columns(const std::vector<std::string>& available, const
         out.push_back(int(it - available.begin()));
     }
     return out;
+}
+
+// ---- schema resolution ----------------------------------------------------------------------------------------------
+namespace {
+
+[[noreturn]] void unresolvable(const std::string& path, const std::string& what) {
+    throw std::runtime_error("schema resolution: " + (path.empty() ? std::string("top-level record") : "field '" + path + "'") + ": " + what);
+}
+
+const char* kind_text(const AvroNode& n) {
+    switch (n.k) {
+        case AK::Null: return "null";
+        case AK::Bool: return "boolean";
+        case AK::Int: return "int";
+        case AK::Long: return "long";
+        case AK::Float: return "float";
+        case AK::Double: return "double";
+        case AK::String: return "string";
+        case AK::Bytes: return "bytes";
+        case AK::Date: return "date";
+        case AK::TsMillis: return "timestamp-millis";
+        case AK::TsMicros: return "timestamp-micros";
+        case AK::TimeMillis: return "time-millis";
+        case AK::TimeMicros: return "time-micros";
+        case AK::Uuid: return "uuid";
+        case AK::DecimalBytes: case AK::DecimalFixed: return "decimal";
+        case AK::Fixed: return "fixed";
+        case AK::Enum: return "enum";
+        case AK::Record: return "record";
+        case AK::Array: return "array";
+        case AK::Map: return "map";
+        case AK::Union: return "union";
+        default: return "unsupported type";
+    }
+}
+
+bool is_logical(AK k) {
+    return k == AK::Date || k == AK::TsMillis || k == AK::TsMicros || k == AK::TimeMillis || k == AK::TimeMicros || k == AK::Uuid ||
+           k == AK::DecimalBytes || k == AK::DecimalFixed;
+}
+
+// ["null", T] or [T, "null"]: T; otherwise nullptr
+const AvroNode* nullable_inner(const AvroNode& n) {
+    if (n.k != AK::Union || n.sub.size() != 2) return nullptr;
+    if (n.sub[0]->k == AK::Null) return n.sub[1].get();
+    if (n.sub[1]->k == AK::Null) return n.sub[0].get();
+    return nullptr;
+}
+
+std::string short_name(const std::string& full) {
+    const size_t dot = full.rfind('.');
+    return dot == std::string::npos ? full : full.substr(dot + 1);
+}
+
+// Named types match when the unqualified names are equal or the reader lists the writer's name among its aliases.
+bool names_match(const AvroNode& w, const AvroNode& r) {
+    if (short_name(w.fullname) == short_name(r.fullname)) return true;
+    for (const std::string& a : r.aliases)
+        if (a == w.fullname || short_name(a) == short_name(w.fullname)) return true;
+    return false;
+}
+
+// Zero wire bytes and no buffers (plan.cpp's zero_sized): a list of such items is never iterated.
+bool takes_no_bytes(const AvroNode& s) {
+    if (s.k == AK::Null) return true;
+    if (s.k == AK::Record) {
+        for (auto& f : s.fields)
+            if (!takes_no_bytes(*f.type)) return false;
+        return true;
+    }
+    return false;
+}
+
+bool json_integer(const Json& j, int64_t lo, int64_t hi, int64_t* out) {
+    if (j.kind != Json::Number || j.str.empty() || j.str.find_first_of(".eE") != std::string::npos) return false;
+    errno = 0;
+    char* end = nullptr;
+    const long long v = std::strtoll(j.str.c_str(), &end, 10);
+    if (errno || !end || *end || v < lo || v > hi) return false;
+    *out = v;
+    return true;
+}
+
+DefaultValue default_of(const AvroNode& t, const Json* j, const std::string& path) {
+    if (!j) unresolvable(path, "the writer's schema has no such field and the reader's has no \"default\" for it");
+    DefaultValue d;
+    const AvroNode* v = &t;
+    // A union's default belongs to its first branch.  A null one is a null of the reader's type, whatever the other
+    // branches are (a null record, list, map, fixed, ...: plan.cpp builds it as a subtree that is never present).
+    if (t.k == AK::Null || (t.k == AK::Union && t.sub[0]->k == AK::Null)) {
+        if (j->kind != Json::Null) unresolvable(path, std::string("the default does not match the field's type (") + (t.k == AK::Null ? "null" : "union whose first branch is null") + ")");
+        d.is_null = true;
+        return d;
+    }
+    if (t.k == AK::Union) {
+        const AvroNode* in = nullable_inner(t);
+        if (!in) unresolvable(path, "default of union is not supported (a non-null default needs [T, \"null\"])");
+        v = in;
+    }
+    switch (v->k) {  // the value of the default: leaves only
+        case AK::Record: case AK::Array: case AK::Map: case AK::Fixed: case AK::DecimalBytes: case AK::DecimalFixed: case AK::Uuid:
+            unresolvable(path, std::string("default of ") + kind_text(*v) + " is not supported");
+        default: break;
+    }
+    auto mismatch = [&]() { unresolvable(path, std::string("the default does not match the field's type (") + kind_text(*v) + ")"); };
+    switch (v->k) {
+        case AK::Bool:
+            if (j->kind != Json::Bool) mismatch();
+            d.i = j->b ? 1 : 0;
+            break;
+        case AK::Int: case AK::Date: case AK::TimeMillis:
+            if (!json_integer(*j, INT32_MIN, INT32_MAX, &d.i)) mismatch();
+            break;
+        case AK::Long: case AK::TsMillis: case AK::TsMicros: case AK::TimeMicros:
+            if (!json_integer(*j, INT64_MIN, INT64_MAX, &d.i)) mismatch();
+            break;
+        case AK::Float: case AK::Double: {
+            if (j->kind != Json::Number) mismatch();
+            char* end = nullptr;
+            d.d = std::strtod(j->str.c_str(), &end);
+            if (!end || *end) mismatch();
+            break;
+        }
+        case AK::String:
+            if (!j->is_string()) mismatch();
+            d.bytes = j->str;
+            break;
+        case AK::Bytes: {  // a JSON string of code points 0-255, one byte each
+            if (!j->is_string()) mismatch();
+            const std::string& u = j->str;
+            for (size_t i = 0; i < u.size();) {
+                const unsigned char c0 = static_cast<unsigned char>(u[i]);
+                if (c0 < 0x80) { d.bytes.push_back(char(c0)); i += 1; continue; }
+                if ((c0 & 0xE0) != 0xC0 || i + 1 >= u.size()) mismatch();   // 2-byte UTF-8 sequences reach U+07FF
+                const unsigned cp = ((c0 & 0x1Fu) << 6) | (static_cast<unsigned char>(u[i + 1]) & 0x3Fu);
+                if (cp > 0xFF) mismatch();
+                d.bytes.push_back(char(cp));
+                i += 2;
+            }
+            break;
+        }
+        case AK::Enum:
+            if (!j->is_string() || std::find(v->symbols.begin(), v->symbols.end(), j->str) == v->symbols.end()) mismatch();
+            d.bytes = j->str;
+            break;
+        default:
+            mismatch();
+    }
+    return d;
+}
+
+Resolution resolve_node(const AvroNode& w, const AvroNode& r, const std::string& path) {
+    Resolution res;
+    res.w = &w;
+    res.r = &r;
+    auto unsupported_pair = [&]() {
+        unresolvable(path, std::string("a writer ") + kind_text(w) + " cannot be read as a reader " + kind_text(r));
+    };
+    if (r.k == AK::Union) {
+        if (const AvroNode* ri = nullable_inner(r)) {
+            if (w.k == AK::Union) {
+                const AvroNode* wi = nullable_inner(w);
+                if (!wi) unresolvable(path, "union branches added, removed or reordered are not supported");
+                res.sub.push_back(resolve_node(*wi, *ri, path));
+            } else {
+                if (w.k == AK::Null) unresolvable(path, "a writer null read as a reader union is not supported");
+                res.sub.push_back(resolve_node(w, *ri, path));
+            }
+            return res;
+        }
+        if (w.k != AK::Union || w.sub.size() != r.sub.size() || nullable_inner(w))
+            unresolvable(path, "union branches added, removed or reordered are not supported");
+        for (size_t i = 0; i < r.sub.size(); ++i) res.sub.push_back(resolve_node(*w.sub[i], *r.sub[i], path));
+        return res;
+    }
+    if (w.k == AK::Union) unresolvable(path, "a writer union read as a reader non-union is not supported");
+    if (w.k != r.k) {
+        if (is_logical(w.k) || is_logical(r.k)) unresolvable(path, std::string("promotions between logical types are not supported (writer ") + kind_text(w) + ", reader " + kind_text(r) + ")");
+        const bool ok = (w.k == AK::Int && (r.k == AK::Long || r.k == AK::Float || r.k == AK::Double)) ||
+                        (w.k == AK::Long && (r.k == AK::Float || r.k == AK::Double)) || (w.k == AK::Float && r.k == AK::Double) ||
+                        (w.k == AK::String && r.k == AK::Bytes) || (w.k == AK::Bytes && r.k == AK::String);
+        if (!ok) unsupported_pair();
+        return res;
+    }
+    switch (r.k) {
+        case AK::Fixed: case AK::DecimalFixed:
+            if (!names_match(w, r)) unresolvable(path, "fixed \"" + w.fullname + "\" does not match \"" + r.fullname + "\"");
+            if (w.size != r.size) unresolvable(path, "fixed sizes differ");
+            if (w.precision != r.precision || w.scale != r.scale) unresolvable(path, "decimal precision or scale differ");
+            return res;
+        case AK::DecimalBytes:
+            if (w.precision != r.precision || w.scale != r.scale) unresolvable(path, "decimal precision or scale differ");
+            return res;
+        case AK::Enum: {
+            if (!names_match(w, r)) unresolvable(path, "enum \"" + w.fullname + "\" does not match \"" + r.fullname + "\"");
+            int dflt = -1;
+            if (r.has_enum_default) dflt = int(std::find(r.symbols.begin(), r.symbols.end(), r.enum_default) - r.symbols.begin());
+            for (const std::string& sym : w.symbols) {
+                const auto it = std::find(r.symbols.begin(), r.symbols.end(), sym);
+                res.sym.push_back(it != r.symbols.end() ? int(it - r.symbols.begin()) : dflt);
+            }
+            return res;
+        }
+        case AK::Record: {
+            if (!names_match(w, r)) unresolvable(path, "record \"" + w.fullname + "\" does not match \"" + r.fullname + "\"");
+            for (const AvroField& rf : r.fields) {
+                const std::string fp = path.empty() ? rf.name : path + "." + rf.name;
+                int src = -1;  // the writer field of the same name, else the one the first matching reader alias names
+                for (size_t i = 0; i < w.fields.size() && src < 0; ++i)
+                    if (w.fields[i].name == rf.name) src = int(i);
+                for (const std::string& a : rf.aliases)
+                    for (size_t i = 0; i < w.fields.size() && src < 0; ++i)
+                        if (w.fields[i].name == a) src = int(i);
+                for (int earlier : res.src)
+                    if (src >= 0 && earlier == src) unresolvable(fp, "writer field '" + w.fields[size_t(src)].name + "' is read by two reader fields");
+                res.src.push_back(src);
+                if (src >= 0) {
+                    res.sub.push_back(resolve_node(*w.fields[size_t(src)].type, *rf.type, fp));
+                } else {
+                    Resolution d;
+                    d.r = rf.type.get();
+                    d.def = default_of(*rf.type, rf.dflt.get(), fp);
+                    res.sub.push_back(std::move(d));
+                }
+            }
+            return res;
+        }
+        case AK::Array: case AK::Map:
+            if (r.k == AK::Array && takes_no_bytes(*w.sub[0]) && !takes_no_bytes(*r.sub[0]))
+                unresolvable(path, "list items that take no wire bytes cannot be read as items that own buffers (DESIGN.md §10)");
+            res.sub.push_back(resolve_node(*w.sub[0], *r.sub[0], path));
+            return res;
+        case AK::Unsupported:
+            unresolvable(path, "unsupported type: " + r.what);
+        default:
+            return res;  // the same primitive / logical type
+    }
+}
+
+}  // namespace
+
+Resolution resolve_schemas(const AvroNode& writer, const AvroNode& reader) {
+    if (writer.k != AK::Record || reader.k != AK::Record) throw std::runtime_error("schema resolution: both schemas must be records");
+    return resolve_node(writer, reader, std::string());
 }
 
 }  // namespace rv

@@ -25,11 +25,14 @@ enum class AK : uint8_t {
 };
 
 struct AvroNode;
+struct Json;
 struct AvroField {
     std::string name;
     std::unique_ptr<AvroNode> type;
     bool has_doc = false;
     std::string doc;
+    std::shared_ptr<const Json> dflt;  // the field's "default" as written (nullptr: none); checked only when a resolution uses it
+    std::vector<std::string> aliases;  // the field's "aliases" (strings only)
 };
 struct AvroNode {
     AK k = AK::Null;
@@ -40,6 +43,8 @@ struct AvroNode {
     std::vector<std::string> aliases;  // namespace-qualified
     std::vector<AvroField> fields;     // record
     std::vector<std::string> symbols;  // enum
+    bool has_enum_default = false;     // enum: "default" (one of the symbols)
+    std::string enum_default;
     std::vector<std::unique_ptr<AvroNode>> sub;  // union variants; array: [items]; map: [values]
     std::string what;                  // Unsupported: which construct
     int32_t size = 0;                  // fixed / decimal on fixed: bytes
@@ -75,5 +80,30 @@ void export_arrow_schema(const std::vector<ArrowField>& fields, ArrowSchema* out
 // Throws std::invalid_argument for an empty list, a repeated name, or a name that is not a field (the message lists the
 // available ones).
 std::vector<int> select_columns(const std::vector<std::string>& available, const std::vector<std::string>& requested);
+
+// ---- schema resolution (rv_schema_resolve): data written with one schema, read as another --------------------------
+// The constant that fills a reader field the writer does not have.
+struct DefaultValue {
+    bool is_null = false;
+    int64_t i = 0;      // boolean, int, long and their logical types
+    double d = 0;       // float, double
+    std::string bytes;  // string, bytes (code points 0-255), enum symbol
+};
+
+// How the writer's node `w` is read as the reader's node `r` (the Avro specification's "Schema Resolution", restricted
+// as DESIGN.md §7 lists).  w == nullptr: a reader record field the writer does not have, filled with `def`.
+struct Resolution {
+    const AvroNode* w = nullptr;
+    const AvroNode* r = nullptr;
+    std::vector<int> src;         // record: for each reader field, the writer field it reads (-1: its default)
+    std::vector<Resolution> sub;  // record: one per reader field; union: one per variant; nullable: [inner]; array / map: [items]
+    std::vector<int> sym;         // enum: for each writer symbol, the reader symbol it becomes (-1: none, the record fails)
+    DefaultValue def;
+};
+
+// The resolution of two top-level records.  Throws std::runtime_error ("schema resolution: field 'a.b': ...") for the
+// first pair outside the rules, naming the reader field's path.  The single place the rules live: the product's plan
+// and the host emulation both build from it.
+Resolution resolve_schemas(const AvroNode& writer, const AvroNode& reader);
 
 }  // namespace rv

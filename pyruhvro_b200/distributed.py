@@ -69,12 +69,13 @@ def _lib():
     return lib
 
 
-def decode_sharded(schema_json: str, d_data, d_offsets, n_local: int, num_chunks: int = 1, *, columns=None):
+def decode_sharded(schema_json: str, d_data, d_offsets, n_local: int, num_chunks: int = 1, *, columns=None, reader_schema=None):
     """This rank's shard -> device-resident result handle (the reference's per-chunk batches; no collective).
-    `columns`: a column projection (top-level field names, pyruhvro_b200.Schema.project)."""
+    `columns`: a column projection (top-level field names, pyruhvro_b200.Schema.project).  `reader_schema`: the schema to
+    read the data as (pyruhvro_b200.Schema.read_as); `schema_json` is the one it was written with."""
     import torch
     from . import _check, _get_or_parse_schema, lib
-    s = _get_or_parse_schema(schema_json, columns)
+    s = _get_or_parse_schema(schema_json, columns, reader_schema)
     h = ctypes.c_void_p()
     _check(lib.rv_decode_device(s.handle, d_data.data_ptr(), d_offsets.data_ptr(), n_local, num_chunks,
                                 torch.cuda.current_stream().cuda_stream, ctypes.byref(h)))
@@ -167,13 +168,13 @@ def gather_result(schema, h, group=None, batch: int = 0):
 
 
 def decode_and_gather(schema_json: str, d_data, d_offsets, n_local: int, group=None, timing: bool = False, to_host: bool = False, *,
-                      columns=None):
+                      columns=None, reader_schema=None):
     """Decode this rank's shard on its GPU, then gather into single RecordBatches on the group leaders.
     Returns a dict: `batches` (pyarrow RecordBatches when to_host, else live rv_result handles freed here), timings."""
     import torch
     from . import _check, _export_batches, lib
     t0 = time.perf_counter()
-    s, h = decode_sharded(schema_json, d_data, d_offsets, n_local, 1, columns=columns)
+    s, h = decode_sharded(schema_json, d_data, d_offsets, n_local, 1, columns=columns, reader_schema=reader_schema)
     torch.cuda.synchronize()
     t1 = time.perf_counter()
     try:
@@ -196,7 +197,9 @@ def decode_and_gather(schema_json: str, d_data, d_offsets, n_local: int, group=N
     return out
 
 
-def decode_sharded_gather(schema_json: str, d_data, d_offsets, n_local: int, group=None, *, columns=None) -> List[pa.RecordBatch]:
+def decode_sharded_gather(schema_json: str, d_data, d_offsets, n_local: int, group=None, *, columns=None,
+                          reader_schema=None) -> List[pa.RecordBatch]:
     """Decode + gather; the group leaders (rank 0 when everything fits one batch) get the gathered RecordBatches in
     pinned host memory, the other ranks an empty list."""
-    return decode_and_gather(schema_json, d_data, d_offsets, n_local, group=group, to_host=True, columns=columns)["batches"]
+    return decode_and_gather(schema_json, d_data, d_offsets, n_local, group=group, to_host=True, columns=columns,
+                             reader_schema=reader_schema)["batches"]

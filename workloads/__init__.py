@@ -73,6 +73,32 @@ NULLABLE_SCHEMA = json.dumps({  # benches/common/mod.rs:67-79
                {"name": "d", "type": ["null", "double"], "default": None}, {"name": "b", "type": ["null", "boolean"], "default": None},
                {"name": "s", "type": ["null", "string"], "default": None}]})
 
+def kafka_v2_schema(enum_symbols=("A", "B", "C", "D"), enum_default=None) -> str:
+    """A reader of KAFKA_SCHEMA data ("Kafka v2", tools/bench_resolve.py): the bench's schema as a later version reads it: phone_numbers dropped, age widened to long, three new
+    fields with defaults, more enum symbols, Address reshaped, created_at first."""
+    enum = {"type": "enum", "name": "enum_col", "symbols": list(enum_symbols)}
+    if enum_default is not None:
+        enum["default"] = enum_default
+    address = {"type": "record", "name": "Address", "fields": [
+        {"name": "city", "type": "string"}, {"name": "street", "type": "string"},
+        {"name": "country", "type": "string", "default": "US"}]}
+    prefs = {"type": "record", "name": "Preferences", "fields": [
+        {"name": "contact_method", "type": ["null", "string"], "default": None}, {"name": "newsletter", "type": "boolean"}]}
+    return json.dumps({"type": "record", "name": "User", "fields": [
+        {"name": "created_at", "type": "long"},
+        {"name": "name", "type": ["null", "string"], "default": None},
+        {"name": "age", "type": ["null", "long"], "default": None},
+        {"name": "emails", "type": {"type": "array", "items": "string"}},
+        {"name": "address", "type": ["null", address], "default": None},
+        {"name": "preferences", "type": ["null", prefs], "default": None},
+        {"name": "status", "type": ["null", "string", "int", "boolean"], "default": None},
+        {"name": "class", "type": enum},
+        {"name": "country", "type": ["null", "string"], "default": None},
+        {"name": "score", "type": "double", "default": 0.0},
+        {"name": "source", "type": "string", "default": "kafka"},
+    ]})
+
+
 CONFIGS = {
     "flat": (2, FLAT_SCHEMA), "kafka": (3, KAFKA_SCHEMA), "wide": (4, WIDE_SCHEMA),
     "array_map": (5, ARRAY_MAP_SCHEMA), "nested": (6, NESTED_SCHEMA), "nullable": (7, NULLABLE_SCHEMA),
