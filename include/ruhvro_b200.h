@@ -34,7 +34,7 @@ struct ArrowDeviceArray; /* Arrow C Device Data Interface */
 
 typedef struct rv_schema rv_schema; /* parsed Avro schema + decode plan; immutable, ref-counted */
 typedef struct rv_result rv_result; /* the k RecordBatches of one decode call */
-typedef struct rv_encoded rv_encoded; /* the k Binary arrays of one encode call */
+typedef struct rv_encoded rv_encoded; /* the k Binary arrays (or the container file) of one encode call */
 
 typedef enum rv_status {
     RV_OK = 0,
@@ -204,9 +204,39 @@ rv_status rv_encode_host(const rv_schema* s, struct ArrowArray* batch, struct Ar
 int64_t rv_encoded_num_chunks(const rv_encoded* r);
 rv_status rv_encoded_export(rv_encoded* r, int64_t chunk, struct ArrowArray* out_array, struct ArrowSchema* out_schema);
 void rv_encoded_free(rv_encoded* r);
-/* CUDA-event timings of the calling thread's last encode, in milliseconds: [0] size kernel, [1] scan, [2] write kernel,
- * [3] upload of the Arrow buffers, [4] download of the datums.  Returns how many entries were written. */
+/* CUDA-event timings of the calling thread's last encode, in milliseconds: [0] size kernel, [1] scan, [2] write kernel
+ * (with the container framing kernel), [3] upload of the Arrow buffers, [4] download of the datums.  Summed over row
+ * groups.  Returns how many entries were written. */
 int rv_last_encode_timings(float* out_ms, int cap);
+
+/* Framed outputs, the write-side mirror of the framed inputs above (extensions: the reference has no such calls).  Both
+ * follow rv_encode_host in everything not stated here: ownership of batch / batch_schema moves to the callee, columns
+ * are matched by name, slices are honoured, errors are the same (the lowest failing row wins), and a projected or
+ * resolved handle is RV_ERR_INVALID.
+ *
+ * Confluent wire format: every datum is preceded by 0x00 and the big-endian u32 schema_id.  Chunking is rv_encode_host's;
+ * chunk i is exported by rv_encoded_export as a Binary array whose element j is the 5-byte header followed by the datum,
+ * and the i32 overflow check of a chunk counts the headers.  schema_id outside [0, 2^32 - 1] is RV_ERR_INVALID. */
+rv_status rv_encode_host_confluent(const rv_schema* s, struct ArrowArray* batch, struct ArrowSchema* batch_schema,
+                                   int64_t num_chunks, int64_t schema_id, rv_encoded** out);
+
+/* One Object Container File of the batch's rows, codec "null":
+ *   "Obj" 1, one metadata map block of 2 + n_meta entries: avro.schema (the exact text `s` was parsed from), avro.codec
+ *   "null", then the caller's pairs in order; the 16-byte `sync` marker; then per block j: zigzag(count), zigzag(byte
+ *   size), the datums of rows [j R, min((j + 1) R, n)), the sync marker (R = block_records).
+ * With no rows the file ends after the header's sync marker; blocks are never empty.  The file is read back by
+ * rv_decode_ocf_host.  The result holds no chunks (rv_encoded_num_chunks is 0): rv_encoded_file returns the file.
+ * RV_ERR_INVALID, before any CUDA call: block_records < 1, a null sync, n_meta < 0, a metadata key that is empty,
+ * starts with "avro." or repeats, a negative value length.  RV_ERR_SCHEMA, before any CUDA call: a schema whose datums
+ * are always empty (records of null fields only), which no container reader takes.  RV_ERR_OVERFLOW: a block whose
+ * datums exceed 2^31 - 1 bytes, with the block's first row.  The file itself may exceed 4 GiB. */
+rv_status rv_encode_ocf_host(const rv_schema* s, struct ArrowArray* batch, struct ArrowSchema* batch_schema,
+                             int64_t block_records, const uint8_t* sync /* 16 bytes */,
+                             const char* const* meta_keys, const uint8_t* const* meta_values,
+                             const int64_t* meta_value_lens, int64_t n_meta, rv_encoded** out);
+/* The whole file of an rv_encode_ocf_host result: one contiguous pinned host buffer owned by `r`.  RV_ERR_INVALID for a
+ * chunked result. */
+rv_status rv_encoded_file(const rv_encoded* r, const uint8_t** data, int64_t* len);
 
 /* ---- multi-GPU: gathering shard-local batches into single RecordBatches ---------------------------------------------
  * Records shard by message; each rank decodes its contiguous range (exactly the reference's per-chunk batches,

@@ -31,7 +31,7 @@ from . import _build
 __all__ = [
     "deserialize_array", "deserialize_array_threaded", "deserialize_array_threaded_spawn",
     "serialize_record_batch", "serialize_record_batch_spawn", "lib", "Schema", "decode_packed", "deserialize_arrow_array",
-    "deserialize_confluent", "deserialize_ocf",
+    "deserialize_confluent", "deserialize_ocf", "serialize_confluent", "serialize_ocf",
 ]
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
@@ -97,6 +97,9 @@ def _bind(L):
     L.rv_result_free.argtypes = [vp]
     L.rv_result_free.restype = None
     L.rv_encode_host.argtypes = [vp, vp, vp, i64, ctypes.POINTER(vp)]
+    L.rv_encode_host_confluent.argtypes = [vp, vp, vp, i64, i64, ctypes.POINTER(vp)]
+    L.rv_encode_ocf_host.argtypes = [vp, vp, vp, i64, vp, vp, vp, vp, i64, ctypes.POINTER(vp)]
+    L.rv_encoded_file.argtypes = [vp, ctypes.POINTER(vp), ctypes.POINTER(i64)]
     L.rv_encoded_num_chunks.restype = i64
     L.rv_encoded_num_chunks.argtypes = [vp]
     L.rv_encoded_export.argtypes = [vp, i64, vp, vp]
@@ -406,18 +409,18 @@ def deserialize_arrow_array(array, schema, num_chunks=1, *, columns=None, reader
     return decode_packed(data, off, n, schema, int(num_chunks), columns=columns, reader_schema=reader_schema)
 
 
-def serialize_record_batch(data, schema, num_chunks):
-    """pyarrow.RecordBatch -> `num_chunks` pyarrow Binary arrays of schemaless Avro datums
-    (src/lib.rs:91-106; ruhvro/src/serialize.rs:38-67), encoded on the GPU (rv_encode_host)."""
-    if not isinstance(data, pa.RecordBatch):
-        raise TypeError("argument 'data': expected a pyarrow.RecordBatch")
-    if num_chunks < 0:
-        raise OverflowError("can't convert negative int to unsigned")
+def _encode(encode_fn, data, schema, *args) -> int:
+    """Exports the RecordBatch through the Arrow C Data Interface (ownership moves to the library) and runs one of the
+    rv_encode_* calls; returns the rv_encoded handle."""
     s = _get_or_parse_schema(schema)
     c_arr, c_sch = _ArrowArray(), _ArrowSchema()
     data._export_to_c(ctypes.addressof(c_arr), ctypes.addressof(c_sch))
     h = ctypes.c_void_p()
-    _check(lib.rv_encode_host(s.handle, ctypes.addressof(c_arr), ctypes.addressof(c_sch), int(num_chunks), ctypes.byref(h)))
+    _check(encode_fn(s.handle, ctypes.addressof(c_arr), ctypes.addressof(c_sch), *args, ctypes.byref(h)))
+    return h.value
+
+
+def _export_chunks(h) -> list:
     try:
         out = []
         for i in range(lib.rv_encoded_num_chunks(h)):
@@ -427,6 +430,69 @@ def serialize_record_batch(data, schema, num_chunks):
         return out
     finally:
         lib.rv_encoded_free(h)
+
+
+def _check_batch(data, num_chunks):
+    if not isinstance(data, pa.RecordBatch):
+        raise TypeError("argument 'data': expected a pyarrow.RecordBatch")
+    if num_chunks < 0:
+        raise OverflowError("can't convert negative int to unsigned")
+
+
+def serialize_record_batch(data, schema, num_chunks):
+    """pyarrow.RecordBatch -> `num_chunks` pyarrow Binary arrays of schemaless Avro datums
+    (src/lib.rs:91-106; ruhvro/src/serialize.rs:38-67), encoded on the GPU (rv_encode_host)."""
+    _check_batch(data, num_chunks)
+    return _export_chunks(_encode(lib.rv_encode_host, data, schema, int(num_chunks)))
+
+
+def serialize_confluent(data, schema, schema_id, num_chunks=1):
+    """pyarrow.RecordBatch -> `num_chunks` pyarrow Binary arrays of Confluent-framed Kafka messages: element i is 0x00,
+    the big-endian u32 `schema_id`, then row i's datum (rv_encode_host_confluent).  The header is written by the encode
+    kernels, so there is no per-message slicing or concatenation in Python.  Chunking is serialize_record_batch's; the
+    messages read back with deserialize_confluent."""
+    _check_batch(data, num_chunks)
+    return _export_chunks(_encode(lib.rv_encode_host_confluent, data, schema, int(num_chunks), int(schema_id)))
+
+
+class _EncodedFile:
+    """Keeps an rv_encoded alive for as long as a pa.Buffer over its file exists."""
+
+    def __init__(self, handle):
+        self.handle = handle
+
+    def __del__(self):
+        h, self.handle = getattr(self, "handle", None), None
+        if h:
+            lib.rv_encoded_free(h)
+
+
+def serialize_ocf(data, schema, block_records=1024, *, sync_marker=None, metadata=None) -> pa.Buffer:
+    """pyarrow.RecordBatch -> one Avro Object Container File (codec "null") as a pa.Buffer over the library's pinned
+    file, without a copy (rv_encode_ocf_host).  The header holds `schema` as avro.schema, avro.codec "null" and the
+    `metadata` pairs (dict[str, bytes]; keys must not be empty or start with "avro."); every block holds `block_records`
+    rows, the last one the rest, and ends with `sync_marker` (16 bytes; default: os.urandom(16)).  deserialize_ocf reads
+    the buffer directly.
+
+    Blocks are the encoder's chunks and its 256-row tiles never span two blocks, so a `block_records` that is not a
+    multiple of 256 leaves lanes idle.  The default 1024 is four full tiles per block, about 120 KB per block of Kafka
+    rows."""
+    _check_batch(data, 0)
+    sync = os.urandom(16) if sync_marker is None else bytes(sync_marker)
+    if len(sync) != 16:
+        raise ValueError(f"sync_marker must be 16 bytes, got {len(sync)}")
+    items = list((metadata or {}).items())
+    keys = [k.encode("utf-8") if isinstance(k, str) else k for k, _ in items]
+    vals = [bytes(v) for _, v in items]
+    n = len(items)
+    c_keys = (ctypes.c_char_p * max(n, 1))(*keys)
+    c_vals = (ctypes.c_char_p * max(n, 1))(*vals)
+    c_lens = (ctypes.c_int64 * max(n, 1))(*[len(v) for v in vals])
+    h = _encode(lib.rv_encode_ocf_host, data, schema, int(block_records), sync, c_keys, c_vals, c_lens, n)
+    owner = _EncodedFile(h)
+    ptr, length = ctypes.c_void_p(), ctypes.c_int64()
+    _check(lib.rv_encoded_file(h, ctypes.byref(ptr), ctypes.byref(length)))
+    return pa.foreign_buffer(ptr.value, length.value, base=owner)
 
 
 def serialize_record_batch_spawn(data, schema, num_chunks):

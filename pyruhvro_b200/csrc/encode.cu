@@ -10,12 +10,18 @@
 // the device; one lane per top-level row walks the nodes in lock step twice — SIZE (bytes this row encodes
 // to; CTA-reduced into per-tile totals), a per-chunk scan (offsets restart at 0 in every output chunk),
 // then WRITE (datum bytes + the BinaryArray's i32 offsets).  Integer/byte work; HBM-bound in principle.
+//
+// Framed outputs, the write-side mirror of the framed inputs: a Confluent-framed encode adds a 5-byte prefix (0x00 + the
+// big-endian u32 schema id) to every row in both passes; an Object Container File encode makes every block one chunk of
+// the same passes, writes the datums of a row group's blocks back to back into one device segment, and a framing kernel
+// puts each block's count and size varints in front of its datums and the sync marker after them.
 #include <cuda_runtime.h>
 
 #include <algorithm>
 #include <atomic>
 #include <array>
 #include <chrono>
+#include <functional>
 #include <mutex>
 #include <cstdio>
 #include <cstdlib>
@@ -67,13 +73,19 @@ struct EncParams {
     uint32_t* tile_base;  // [n_tiles]
     unsigned long long* err;
     uint8_t* const* out_data;   // [k]
-    int32_t* const* out_offsets;  // [k]
+    int32_t* const* out_offsets;  // [k] (Object Container Files: unused)
     uint32_t stage_cap;   // bytes of dynamic shared memory in which a tile's datums are assembled
+    uint32_t schema_id;   // Confluent prefix
 };
 
 namespace {
 
 enum EncErr : uint32_t { EE_ENUM = RV_ERR_ENUM, EE_BRANCH = RV_ERR_BRANCH, EE_OVERFLOW = RV_ERR_OVERFLOW };
+
+// What the write pass produces: bare datums + Binary offsets, Confluent-framed datums + Binary offsets, or the datums of
+// container blocks (no offsets: the framing kernel delimits the blocks).
+enum EncOut : int { EO_BINARY = 0, EO_CONFLUENT = 1, EO_OCF = 2 };
+constexpr uint32_t kConfluentHeader = 5;
 
 struct EncCtx {
     const ENode* nodes;
@@ -235,6 +247,8 @@ __device__ __forceinline__ void enc_init(EncCtx& c, const EncParams& p) {
     c.pm = 1u; c.usel = 0; c.err = 0; c.size = 0; c.out = nullptr;
 }
 
+// PREFIX: bytes written in front of every datum (0, or kConfluentHeader); they count towards the row, tile and chunk sizes.
+template <uint32_t PREFIX>
 __global__ void __launch_bounds__(kBlock) encode_size_kernel(const EncParams p) {
     int chunk, nrec, local; int64_t r0;
     enc_tile(p, blockIdx.x, &chunk, &r0, &nrec, &local);
@@ -242,6 +256,7 @@ __global__ void __launch_bounds__(kBlock) encode_size_kernel(const EncParams p) 
     EncCtx c;
     enc_init(c, p);
     if (tid < nrec) {
+        c.size = PREFIX;
         enc_range<0, 0>(c, 0, p.n_nodes, p.row_base + r0 + tid);
         if (c.err) atomicMin(p.err, (static_cast<unsigned long long>(p.row_base + r0 + tid) << 8) | c.err);
         p.row_size[r0 + tid] = c.size;
@@ -259,6 +274,7 @@ __global__ void __launch_bounds__(kBlock) encode_size_kernel(const EncParams p) 
     }
 }
 
+template <int OUT>
 __global__ void __launch_bounds__(kBlock) encode_write_kernel(const EncParams p) {
     int chunk, nrec, local; int64_t r0;
     enc_tile(p, blockIdx.x, &chunk, &r0, &nrec, &local);
@@ -281,13 +297,21 @@ __global__ void __launch_bounds__(kBlock) encode_write_kernel(const EncParams p)
     const uint32_t galign = uint32_t(reinterpret_cast<uintptr_t>(gout) & 15u);
     const bool staged = tile_total + galign <= p.stage_cap;
     if (tid < nrec) {
-        int32_t* offs = p.out_offsets[chunk];
-        const int64_t i = int64_t(local) * kBlock + tid;  // row inside the chunk
-        if (i == 0) offs[0] = 0;
-        offs[i + 1] = int32_t(off + sz);
+        if (OUT != EO_OCF) {
+            int32_t* offs = p.out_offsets[chunk];
+            const int64_t i = int64_t(local) * kBlock + tid;  // row inside the chunk
+            if (i == 0) offs[0] = 0;
+            offs[i + 1] = int32_t(off + sz);
+        }
         EncCtx c;
         enc_init(c, p);
         c.out = staged ? enc_smem + galign + (off - tile_base) : p.out_data[chunk] + off;
+        if (OUT == EO_CONFLUENT) {  // magic byte, then the schema id big-endian
+            c.out[0] = 0;
+            c.out[1] = uint8_t(p.schema_id >> 24); c.out[2] = uint8_t(p.schema_id >> 16);
+            c.out[3] = uint8_t(p.schema_id >> 8); c.out[4] = uint8_t(p.schema_id);
+            c.out += kConfluentHeader;
+        }
         enc_range<1, 0>(c, 0, p.n_nodes, p.row_base + r0 + tid);
     }
     if (staged) {
@@ -336,6 +360,26 @@ __global__ void encode_scan_kernel(const EncParams p, unsigned long long* chunk_
     __syncthreads();
     unsigned long long run = s_part[warp] + (incl - local);
     for (int i = a; i < b; ++i) { p.tile_base[i] = uint32_t(run); run += p.tile_agg[i]; }
+}
+
+struct SyncMarker { uint8_t b[16]; };
+
+// Object Container File blocks (one thread per block = chunk j): the block's record count and datum size as zigzag
+// varints right in front of its datums (p.out_data[j], placed by the host so that exactly these bytes fit), and the sync
+// marker right after them.  Runs after the write kernel, which writes only inside [out_data[j], out_data[j] + size).
+__global__ void ocf_frame_kernel(const EncParams p, const unsigned long long* block_bytes, const SyncMarker sync) {
+    const int j = int(blockIdx.x * blockDim.x + threadIdx.x);
+    if (j >= p.k) return;
+    const int64_t count = (j == p.k - 1) ? p.n - int64_t(j) * p.chunk_rows : p.chunk_rows;
+    const int64_t size = int64_t(block_bytes[j]);
+    EncCtx c;
+    enc_init(c, p);
+    put_long<0>(c, count);
+    put_long<0>(c, size);
+    c.out = p.out_data[j] - c.size;
+    put_long<1>(c, count);
+    put_long<1>(c, size);
+    for (int i = 0; i < 16; ++i) c.out[size + i] = sync.b[i];
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -563,10 +607,14 @@ extern "C" const void* rv_schema_avro_root(const rv_schema* s);
 extern "C" int rv_schema_is_projection(const rv_schema* s);
 extern "C" void rv_set_last_error(const char* msg);
 
+extern "C" const char* rv_internal_schema_json(const rv_schema* s, size_t* len);
+
 struct rv_encoded {
     struct Chunk { void* host = nullptr; int64_t rows = 0, data_bytes = 0; };
     std::vector<Chunk> chunks;  // host: [offsets (rows+1)*4, padded to 64][data]
     std::vector<std::shared_ptr<void>> keep;
+    const uint8_t* file = nullptr;  // an Object Container File encode: the whole file (no chunks; keep[0] owns it)
+    int64_t file_len = 0;
 };
 
 namespace {
@@ -600,26 +648,38 @@ extern "C" int rv_last_encode_timings(float* out_ms, int cap) {
     return n;
 }
 
-// One row group of the batch — chunks [c0, c1), rows [g0, g1) — on its own stream: upload of the buffer windows its rows
-// reach, size -> scan -> write, download of its chunks.  Returns a status; the message goes to *msg (worker threads have
-// their own thread-local error string).
-static rv_status encode_group(const AvroNode* top, const ArrowArray* batch, const ArrowSchema* batch_schema, int64_t g0, int64_t g1,
-                              int c0, int c1, int64_t chunk_rows, cudaStream_t stream, rv_encoded* res, float* ms5,
-                              std::string* msg) {
-#define GRP_CUDA(expr)                                                                                   \
-    do {                                                                                                 \
-        cudaError_t e_ = (expr);                                                                         \
-        if (e_ != cudaSuccess) { *msg = std::string(#expr) + ": " + cudaGetErrorString(e_); cudaStreamSynchronize(stream); (void)cudaGetLastError(); return RV_ERR_CUDA; } \
-    } while (0)
-    EncBuilder b;
-    try {
-        b.record_children(*top, batch, batch_schema, batch->offset, 1, 0, 0, g0, g1);
-    } catch (const std::exception& e) {
-        *msg = e.what();
-        return RV_ERR_INVALID;
-    }
-    const int64_t n = g1 - g0;
-    const int k = c1 - c0;
+}  // extern "C"
+
+// zigzag varint (write_zigzag_long, fast_encode.rs:585-593) on the host: the container header, and the block header lengths
+// that place each block's datums in its row group's segment
+static int zz_len(int64_t v) {
+    unsigned long long z = (static_cast<unsigned long long>(v) << 1) ^ static_cast<unsigned long long>(v >> 63);
+    int n = 1;
+    while (z >= 0x80) { z >>= 7; ++n; }
+    return n;
+}
+static void put_zz(std::string& o, int64_t v) {
+    unsigned long long z = (static_cast<unsigned long long>(v) << 1) ^ static_cast<unsigned long long>(v >> 63);
+    while (z >= 0x80) { o.push_back(char((z & 0x7F) | 0x80)); z >>= 7; }
+    o.push_back(char(z));
+}
+
+// One row group of the batch — chunks [c0, c1), rows [g0, g1) — on its own stream.  measure(): upload of the buffer windows
+// its rows reach, size -> scan, read back of the chunk totals.  Then either write_chunks() (Binary arrays: per chunk
+// [offsets][data] on the device, one download each) or write_blocks() (container blocks: one device segment of the
+// group's framed blocks, one download into the file).  A status's message goes to *msg (worker threads have their own
+// thread-local error string).
+struct EncGroup {
+    const AvroNode* top;
+    const ArrowArray* batch;
+    const ArrowSchema* batch_schema;
+    int64_t g0, g1, chunk_rows;
+    int c0, c1, out;  // out: EncOut
+    uint32_t schema_id;
+    cudaStream_t stream;
+    float* ms5;
+    std::string* msg;
+
     struct Ev {
         cudaEvent_t e[8] = {};
         Ev() { for (auto& x : e) if (cudaEventCreate(&x) != cudaSuccess) x = nullptr; }
@@ -627,127 +687,151 @@ static rv_status encode_group(const AvroNode* top, const ArrowArray* batch, cons
         void rec(int i, cudaStream_t st) { if (e[i]) cudaEventRecord(e[i], st); }
         float ms(int a, int b_) { float t = 0; if (e[a] && e[b_] && cudaEventElapsedTime(&t, e[a], e[b_]) == cudaSuccess) return t; (void)cudaGetLastError(); return 0; }
     } ev;
-
-    // ---- upload the windows of the Arrow buffers this group's rows reach (one device arena) ----
-    size_t total = 0;
-    std::vector<size_t> boff(b.bufs.size()), blo(b.bufs.size());
-    for (size_t i = 0; i < b.bufs.size(); ++i) {
-        blo[i] = b.bufs[i].lo & ~size_t(63);                 // windows start on a 64-byte boundary of the source buffer
-        boff[i] = total;
-        total += (b.bufs[i].hi - blo[i] + 8 + 63) & ~size_t(63);
-    }
-    DevMem d_in, d_nodes, d_symoff, d_symbytes, d_rowsize, d_agg, d_base, d_err, d_tot, d_ptrs;
-    GRP_CUDA(d_in.alloc(total));
-    ev.rec(0, stream);
-    // Buffers in ordinary pageable memory are staged through a pinned arena in 16 MiB pieces (a direct copy runs at a
-    // fraction of PCIe speed); pinned / registered buffers — e.g. batches this library decoded — go direct.
-    bool pageable = false;
-    for (size_t i = 0; i < b.bufs.size() && !pageable; ++i) {
-        if (b.bufs[i].hi - blo[i] < (size_t(1) << 20)) continue;
-        cudaPointerAttributes at{};
-        if (cudaPointerGetAttributes(&at, b.bufs[i].ptr) != cudaSuccess) { (void)cudaGetLastError(); pageable = true; }
-        else pageable = at.type == cudaMemoryTypeUnregistered;
-    }
+    EncBuilder b;
+    DevMem d_in, d_nodes, d_symoff, d_symbytes, d_rowsize, d_agg, d_base, d_err, d_tot, d_ptrs, d_seg;
     std::shared_ptr<void> h_in_keep;
-    uint8_t* h_in = nullptr;
-    if (pageable && total >= (size_t(4) << 20)) {
-        h_in = static_cast<uint8_t*>(rv_host_alloc(total));
-        if (!h_in) { *msg = "pinned staging allocation failed"; return RV_ERR_CUDA; }
-        h_in_keep = std::shared_ptr<void>(h_in, [](void* q) { rv_host_free(q); });
-    }
-    const size_t kPiece = size_t(16) << 20;
-    for (size_t i = 0; i < b.bufs.size(); ++i) {
-        const uint8_t* src = static_cast<const uint8_t*>(b.bufs[i].ptr) + blo[i];
-        const size_t bytes = b.bufs[i].hi - blo[i];
-        uint8_t* dst = static_cast<uint8_t*>(d_in.p) + boff[i];
-        for (size_t o = 0; o < bytes; o += kPiece) {
-            const size_t len = std::min(kPiece, bytes - o);
-            const uint8_t* from = src + o;
-            if (h_in) { std::memcpy(h_in + boff[i] + o, from, len); from = h_in + boff[i] + o; }
-            GRP_CUDA(cudaMemcpyAsync(dst + o, from, len, cudaMemcpyHostToDevice, stream));
-        }
-    }
-    for (size_t i = 0; i < b.nodes.size(); ++i) {
-        // device address of the buffer's byte 0 (the window starts at byte blo): nodes keep indexing absolutely
-        auto fix = [&](int ref) -> const uint8_t* { return ref < 0 ? nullptr : static_cast<const uint8_t*>(d_in.p) + boff[size_t(ref)] - blo[size_t(ref)]; };
-        b.nodes[i].validity = fix(b.ref_v[i]);
-        b.nodes[i].buf_a = fix(b.ref_a[i]);
-        b.nodes[i].buf_b = fix(b.ref_b[i]);
-    }
-    GRP_CUDA(d_nodes.alloc(b.nodes.size() * sizeof(ENode)));
-    GRP_CUDA(cudaMemcpyAsync(d_nodes.p, b.nodes.data(), b.nodes.size() * sizeof(ENode), cudaMemcpyHostToDevice, stream));
-    GRP_CUDA(d_symoff.alloc(b.sym_off.size() * 4));
-    GRP_CUDA(d_symbytes.alloc(b.sym_bytes.size()));
-    if (!b.sym_off.empty()) GRP_CUDA(cudaMemcpyAsync(d_symoff.p, b.sym_off.data(), b.sym_off.size() * 4, cudaMemcpyHostToDevice, stream));
-    if (!b.sym_bytes.empty()) GRP_CUDA(cudaMemcpyAsync(d_symbytes.p, b.sym_bytes.data(), b.sym_bytes.size(), cudaMemcpyHostToDevice, stream));
-    ev.rec(1, stream);
-
     EncParams p{};
-    p.nodes = static_cast<const ENode*>(d_nodes.p); p.n_nodes = int32_t(b.nodes.size());
-    p.sym_off = static_cast<const int32_t*>(d_symoff.p); p.sym_bytes = static_cast<const uint8_t*>(d_symbytes.p);
-    p.n = n; p.row_base = g0; p.chunk_rows = chunk_rows; p.k = k;
-    const int64_t tpc = std::max<int64_t>(1, (chunk_rows + kBlock - 1) / kBlock);
-    const int64_t last_rows = n - chunk_rows * (k - 1);
-    const int64_t n_tiles = n > 0 ? tpc * (k - 1) + (last_rows + kBlock - 1) / kBlock : 0;
-    p.tiles_per_chunk = int32_t(tpc); p.n_tiles = int32_t(n_tiles);
-    std::vector<unsigned long long> chunk_tot(static_cast<size_t>(k), 0ull);
+    int64_t n = 0, n_tiles = 0;
+    int k = 0;
+    std::vector<unsigned long long> chunk_tot;
     unsigned long long max_tile = 0;
-    if (n > 0) {
-        GRP_CUDA(d_rowsize.alloc(size_t(n) * 4));
-        GRP_CUDA(d_agg.alloc(size_t(n_tiles) * 4));
-        GRP_CUDA(d_base.alloc(size_t(n_tiles) * 4));
-        GRP_CUDA(d_err.alloc(16));
-        GRP_CUDA(d_tot.alloc(size_t(k) * 8));
-        GRP_CUDA(cudaMemsetAsync(d_err.p, 0xFF, 8, stream));
-        p.row_size = static_cast<uint32_t*>(d_rowsize.p); p.tile_agg = static_cast<uint32_t*>(d_agg.p);
-        p.tile_base = static_cast<uint32_t*>(d_base.p); p.err = static_cast<unsigned long long*>(d_err.p);
-        encode_size_kernel<<<unsigned(n_tiles), kBlock, 0, stream>>>(p);
-        ev.rec(2, stream);
-        int thr = 32;
-        while (thr < 1024 && thr < tpc) thr <<= 1;
-        encode_scan_kernel<<<unsigned(k), thr, 0, stream>>>(p, static_cast<unsigned long long*>(d_tot.p));
-        GRP_CUDA(cudaMemsetAsync(static_cast<uint8_t*>(d_err.p) + 8, 0, 8, stream));
-        encode_tile_max_kernel<<<std::max(1, std::min(int((n_tiles + 255) / 256), 592)), 256, 0, stream>>>(p, static_cast<unsigned long long*>(d_err.p) + 1);
-        GRP_CUDA(cudaGetLastError());
-        ev.rec(3, stream);
-        unsigned long long err_word = ~0ull;
-        GRP_CUDA(cudaMemcpyAsync(&max_tile, static_cast<uint8_t*>(d_err.p) + 8, 8, cudaMemcpyDeviceToHost, stream));
-        GRP_CUDA(cudaMemcpyAsync(&err_word, d_err.p, 8, cudaMemcpyDeviceToHost, stream));
-        GRP_CUDA(cudaMemcpyAsync(chunk_tot.data(), d_tot.p, size_t(k) * 8, cudaMemcpyDeviceToHost, stream));
-        GRP_CUDA(cudaStreamSynchronize(stream));
-        if (err_word != ~0ull) {
-            const uint32_t code = uint32_t(err_word & 0xFF);
-            const std::string what = code == EE_ENUM ? "fast_encode: enum symbol not in schema"
-                                     : code == EE_BRANCH ? "fast_encode: union type_id out of range"
-                                                         : "Arrow i32 offset overflow: a chunk's datums exceed 2 GiB";
-            *msg = what + " (row " + std::to_string(err_word >> 8) + ")";
-            return rv_status(code);
+    std::vector<uint8_t*> h_data;
+    std::vector<int32_t*> h_offs;
+
+    EncGroup(const AvroNode* top_, const ArrowArray* batch_, const ArrowSchema* bs, int64_t g0_, int64_t g1_, int c0_, int c1_,
+             int64_t chunk_rows_, int out_, uint32_t schema_id_, cudaStream_t stream_, float* ms5_, std::string* msg_)
+        : top(top_), batch(batch_), batch_schema(bs), g0(g0_), g1(g1_), chunk_rows(chunk_rows_), c0(c0_), c1(c1_), out(out_),
+          schema_id(schema_id_), stream(stream_), ms5(ms5_), msg(msg_) {}
+
+#define GRP_CUDA(expr)                                                                                   \
+    do {                                                                                                 \
+        cudaError_t e_ = (expr);                                                                         \
+        if (e_ != cudaSuccess) { *msg = std::string(#expr) + ": " + cudaGetErrorString(e_); cudaStreamSynchronize(stream); (void)cudaGetLastError(); return RV_ERR_CUDA; } \
+    } while (0)
+
+    rv_status measure() {
+        try {
+            b.record_children(*top, batch, batch_schema, batch->offset, 1, 0, 0, g0, g1);
+        } catch (const std::exception& e) {
+            *msg = e.what();
+            return RV_ERR_INVALID;
         }
+        n = g1 - g0;
+        k = c1 - c0;
+
+        // ---- upload the windows of the Arrow buffers this group's rows reach (one device arena) ----
+        size_t total = 0;
+        std::vector<size_t> boff(b.bufs.size()), blo(b.bufs.size());
+        for (size_t i = 0; i < b.bufs.size(); ++i) {
+            blo[i] = b.bufs[i].lo & ~size_t(63);                 // windows start on a 64-byte boundary of the source buffer
+            boff[i] = total;
+            total += (b.bufs[i].hi - blo[i] + 8 + 63) & ~size_t(63);
+        }
+        GRP_CUDA(d_in.alloc(total));
+        ev.rec(0, stream);
+        // Buffers in ordinary pageable memory are staged through a pinned arena in 16 MiB pieces (a direct copy runs at a
+        // fraction of PCIe speed); pinned / registered buffers — e.g. batches this library decoded — go direct.
+        bool pageable = false;
+        for (size_t i = 0; i < b.bufs.size() && !pageable; ++i) {
+            if (b.bufs[i].hi - blo[i] < (size_t(1) << 20)) continue;
+            cudaPointerAttributes at{};
+            if (cudaPointerGetAttributes(&at, b.bufs[i].ptr) != cudaSuccess) { (void)cudaGetLastError(); pageable = true; }
+            else pageable = at.type == cudaMemoryTypeUnregistered;
+        }
+        uint8_t* h_in = nullptr;
+        if (pageable && total >= (size_t(4) << 20)) {
+            h_in = static_cast<uint8_t*>(rv_host_alloc(total));
+            if (!h_in) { *msg = "pinned staging allocation failed"; return RV_ERR_CUDA; }
+            h_in_keep = std::shared_ptr<void>(h_in, [](void* q) { rv_host_free(q); });
+        }
+        const size_t kPiece = size_t(16) << 20;
+        for (size_t i = 0; i < b.bufs.size(); ++i) {
+            const uint8_t* src = static_cast<const uint8_t*>(b.bufs[i].ptr) + blo[i];
+            const size_t bytes = b.bufs[i].hi - blo[i];
+            uint8_t* dst = static_cast<uint8_t*>(d_in.p) + boff[i];
+            for (size_t o = 0; o < bytes; o += kPiece) {
+                const size_t len = std::min(kPiece, bytes - o);
+                const uint8_t* from = src + o;
+                if (h_in) { std::memcpy(h_in + boff[i] + o, from, len); from = h_in + boff[i] + o; }
+                GRP_CUDA(cudaMemcpyAsync(dst + o, from, len, cudaMemcpyHostToDevice, stream));
+            }
+        }
+        for (size_t i = 0; i < b.nodes.size(); ++i) {
+            // device address of the buffer's byte 0 (the window starts at byte blo): nodes keep indexing absolutely
+            auto fix = [&](int ref) -> const uint8_t* { return ref < 0 ? nullptr : static_cast<const uint8_t*>(d_in.p) + boff[size_t(ref)] - blo[size_t(ref)]; };
+            b.nodes[i].validity = fix(b.ref_v[i]);
+            b.nodes[i].buf_a = fix(b.ref_a[i]);
+            b.nodes[i].buf_b = fix(b.ref_b[i]);
+        }
+        GRP_CUDA(d_nodes.alloc(b.nodes.size() * sizeof(ENode)));
+        GRP_CUDA(cudaMemcpyAsync(d_nodes.p, b.nodes.data(), b.nodes.size() * sizeof(ENode), cudaMemcpyHostToDevice, stream));
+        GRP_CUDA(d_symoff.alloc(b.sym_off.size() * 4));
+        GRP_CUDA(d_symbytes.alloc(b.sym_bytes.size()));
+        if (!b.sym_off.empty()) GRP_CUDA(cudaMemcpyAsync(d_symoff.p, b.sym_off.data(), b.sym_off.size() * 4, cudaMemcpyHostToDevice, stream));
+        if (!b.sym_bytes.empty()) GRP_CUDA(cudaMemcpyAsync(d_symbytes.p, b.sym_bytes.data(), b.sym_bytes.size(), cudaMemcpyHostToDevice, stream));
+        ev.rec(1, stream);
+
+        p.nodes = static_cast<const ENode*>(d_nodes.p); p.n_nodes = int32_t(b.nodes.size());
+        p.sym_off = static_cast<const int32_t*>(d_symoff.p); p.sym_bytes = static_cast<const uint8_t*>(d_symbytes.p);
+        p.n = n; p.row_base = g0; p.chunk_rows = chunk_rows; p.k = k; p.schema_id = schema_id;
+        const int64_t tpc = std::max<int64_t>(1, (chunk_rows + kBlock - 1) / kBlock);
+        const int64_t last_rows = n - chunk_rows * (k - 1);
+        n_tiles = n > 0 ? tpc * (k - 1) + (last_rows + kBlock - 1) / kBlock : 0;
+        p.tiles_per_chunk = int32_t(tpc); p.n_tiles = int32_t(n_tiles);
+        chunk_tot.assign(static_cast<size_t>(k), 0ull);
+        if (n > 0) {
+            GRP_CUDA(d_rowsize.alloc(size_t(n) * 4));
+            GRP_CUDA(d_agg.alloc(size_t(n_tiles) * 4));
+            GRP_CUDA(d_base.alloc(size_t(n_tiles) * 4));
+            GRP_CUDA(d_err.alloc(16));
+            GRP_CUDA(d_tot.alloc(size_t(k) * 8));
+            GRP_CUDA(cudaMemsetAsync(d_err.p, 0xFF, 8, stream));
+            p.row_size = static_cast<uint32_t*>(d_rowsize.p); p.tile_agg = static_cast<uint32_t*>(d_agg.p);
+            p.tile_base = static_cast<uint32_t*>(d_base.p); p.err = static_cast<unsigned long long*>(d_err.p);
+            if (out == EO_CONFLUENT) encode_size_kernel<kConfluentHeader><<<unsigned(n_tiles), kBlock, 0, stream>>>(p);
+            else encode_size_kernel<0><<<unsigned(n_tiles), kBlock, 0, stream>>>(p);
+            ev.rec(2, stream);
+            int thr = 32;
+            while (thr < 1024 && thr < tpc) thr <<= 1;
+            encode_scan_kernel<<<unsigned(k), thr, 0, stream>>>(p, static_cast<unsigned long long*>(d_tot.p));
+            GRP_CUDA(cudaMemsetAsync(static_cast<uint8_t*>(d_err.p) + 8, 0, 8, stream));
+            encode_tile_max_kernel<<<std::max(1, std::min(int((n_tiles + 255) / 256), 592)), 256, 0, stream>>>(p, static_cast<unsigned long long*>(d_err.p) + 1);
+            GRP_CUDA(cudaGetLastError());
+            ev.rec(3, stream);
+            unsigned long long err_word = ~0ull;
+            GRP_CUDA(cudaMemcpyAsync(&max_tile, static_cast<uint8_t*>(d_err.p) + 8, 8, cudaMemcpyDeviceToHost, stream));
+            GRP_CUDA(cudaMemcpyAsync(&err_word, d_err.p, 8, cudaMemcpyDeviceToHost, stream));
+            GRP_CUDA(cudaMemcpyAsync(chunk_tot.data(), d_tot.p, size_t(k) * 8, cudaMemcpyDeviceToHost, stream));
+            GRP_CUDA(cudaStreamSynchronize(stream));
+            if (err_word != ~0ull) {
+                const uint32_t code = uint32_t(err_word & 0xFF);
+                const std::string what = code == EE_ENUM ? "fast_encode: enum symbol not in schema"
+                                         : code == EE_BRANCH ? "fast_encode: union type_id out of range"
+                                         : out == EO_OCF ? "Object Container File block overflow: a block's datums exceed 2 GiB"
+                                                         : "Arrow i32 offset overflow: a chunk's datums exceed 2 GiB";
+                *msg = what + " (row " + std::to_string(err_word >> 8) + ")";
+                return rv_status(code);
+            }
+        }
+        return RV_OK;
     }
-    // ---- outputs: per chunk [offsets][data] on the device, then one D2H per chunk into pinned memory ----
-    std::vector<DevMem> d_out(static_cast<size_t>(k));
-    std::vector<uint8_t*> h_data(static_cast<size_t>(k), nullptr);
-    std::vector<int32_t*> h_offs(static_cast<size_t>(k), nullptr);
-    std::vector<size_t> off_bytes(static_cast<size_t>(k), 0);
-    for (int j = 0; j < k; ++j) {
-        auto& c = res->chunks[size_t(c0 + j)];
-        c.data_bytes = int64_t(chunk_tot[size_t(j)]);
-        off_bytes[size_t(j)] = (size_t(c.rows + 1) * 4 + 63) & ~size_t(63);
-        GRP_CUDA(d_out[size_t(j)].alloc(off_bytes[size_t(j)] + size_t(c.data_bytes) + 64));
-        h_offs[size_t(j)] = static_cast<int32_t*>(d_out[size_t(j)].p);
-        h_data[size_t(j)] = static_cast<uint8_t*>(d_out[size_t(j)].p) + off_bytes[size_t(j)];
-        if (c.rows == 0) GRP_CUDA(cudaMemsetAsync(d_out[size_t(j)].p, 0, 64, stream));
+
+    // records of block (chunk) j of the group
+    int64_t rows_of(int j) const { return j == k - 1 ? n - chunk_rows * (k - 1) : chunk_rows; }
+
+    // bytes of the group's part of a container file: every block's count and size varints, datums and sync marker
+    int64_t file_bytes() const {
+        int64_t t = 0;
+        for (int j = 0; j < k; ++j) t += zz_len(rows_of(j)) + zz_len(int64_t(chunk_tot[size_t(j)])) + int64_t(chunk_tot[size_t(j)]) + 16;
+        return t;
     }
-    if (n > 0) {
-        GRP_CUDA(d_ptrs.alloc(size_t(k) * 16));
-        GRP_CUDA(cudaMemcpyAsync(d_ptrs.p, h_data.data(), size_t(k) * 8, cudaMemcpyHostToDevice, stream));
-        GRP_CUDA(cudaMemcpyAsync(static_cast<uint8_t*>(d_ptrs.p) + size_t(k) * 8, h_offs.data(), size_t(k) * 8, cudaMemcpyHostToDevice, stream));
-        p.out_data = static_cast<uint8_t* const*>(d_ptrs.p);
-        p.out_offsets = reinterpret_cast<int32_t* const*>(static_cast<uint8_t*>(d_ptrs.p) + size_t(k) * 8);
+
+    template <int OUT>
+    rv_status launch_write() {
         // staging area: the largest tile (+ alignment), capped so at least two CTAs share an SM
         size_t stage = std::min<size_t>(size_t(max_tile) + 32, 100 * 1024);
         stage = (stage + 63) & ~size_t(63);
-        {   // function attributes are per device
+        {   // function attributes are per device (and per instantiation)
             static std::mutex attr_mu;
             static std::vector<char> attr_set;
             int dev_now = 0;
@@ -755,49 +839,146 @@ static rv_status encode_group(const AvroNode* top, const ArrowArray* batch, cons
             std::lock_guard<std::mutex> g(attr_mu);
             if (attr_set.size() <= size_t(dev_now)) attr_set.resize(size_t(dev_now) + 1, 0);
             if (!attr_set[size_t(dev_now)]) {
-                GRP_CUDA(cudaFuncSetAttribute(encode_write_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 112 * 1024));
-                GRP_CUDA(cudaFuncSetAttribute(encode_write_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
+                GRP_CUDA(cudaFuncSetAttribute(encode_write_kernel<OUT>, cudaFuncAttributeMaxDynamicSharedMemorySize, 112 * 1024));
+                GRP_CUDA(cudaFuncSetAttribute(encode_write_kernel<OUT>, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
                 attr_set[size_t(dev_now)] = 1;
             }
         }
         p.stage_cap = uint32_t(stage);
         ev.rec(4, stream);
-        encode_write_kernel<<<unsigned(n_tiles), kBlock, stage, stream>>>(p);
+        encode_write_kernel<OUT><<<unsigned(n_tiles), kBlock, stage, stream>>>(p);
+        return RV_OK;
+    }
+
+    void record_times() {
+        ms5[3] = ev.ms(0, 1);
+        ms5[4] = ev.ms(6, 7);
+        if (n > 0) { ms5[0] = ev.ms(1, 2); ms5[1] = ev.ms(2, 3); ms5[2] = ev.ms(4, 5); }
+    }
+
+    // ---- outputs: per chunk [offsets][data] on the device, then one D2H per chunk into pinned memory ----
+    rv_status write_chunks(rv_encoded* res) {
+        std::vector<DevMem> d_out(static_cast<size_t>(k));
+        h_data.assign(static_cast<size_t>(k), nullptr);
+        h_offs.assign(static_cast<size_t>(k), nullptr);
+        std::vector<size_t> off_bytes(static_cast<size_t>(k), 0);
+        for (int j = 0; j < k; ++j) {
+            auto& c = res->chunks[size_t(c0 + j)];
+            c.data_bytes = int64_t(chunk_tot[size_t(j)]);
+            off_bytes[size_t(j)] = (size_t(c.rows + 1) * 4 + 63) & ~size_t(63);
+            GRP_CUDA(d_out[size_t(j)].alloc(off_bytes[size_t(j)] + size_t(c.data_bytes) + 64));
+            h_offs[size_t(j)] = static_cast<int32_t*>(d_out[size_t(j)].p);
+            h_data[size_t(j)] = static_cast<uint8_t*>(d_out[size_t(j)].p) + off_bytes[size_t(j)];
+            if (c.rows == 0) GRP_CUDA(cudaMemsetAsync(d_out[size_t(j)].p, 0, 64, stream));
+        }
+        if (n > 0) {
+            GRP_CUDA(d_ptrs.alloc(size_t(k) * 16));
+            GRP_CUDA(cudaMemcpyAsync(d_ptrs.p, h_data.data(), size_t(k) * 8, cudaMemcpyHostToDevice, stream));
+            GRP_CUDA(cudaMemcpyAsync(static_cast<uint8_t*>(d_ptrs.p) + size_t(k) * 8, h_offs.data(), size_t(k) * 8, cudaMemcpyHostToDevice, stream));
+            p.out_data = static_cast<uint8_t* const*>(d_ptrs.p);
+            p.out_offsets = reinterpret_cast<int32_t* const*>(static_cast<uint8_t*>(d_ptrs.p) + size_t(k) * 8);
+            const rv_status st = out == EO_CONFLUENT ? launch_write<EO_CONFLUENT>() : launch_write<EO_BINARY>();
+            if (st) return st;
+            ev.rec(5, stream);
+            GRP_CUDA(cudaGetLastError());
+        }
+        ev.rec(6, stream);
+        for (int j = 0; j < k; ++j) {
+            auto& c = res->chunks[size_t(c0 + j)];
+            const size_t bytes = off_bytes[size_t(j)] + size_t(c.data_bytes);
+            void* h = rv_host_alloc(bytes + 64);
+            if (!h) { *msg = "pinned allocation of an output chunk failed"; cudaStreamSynchronize(stream); return RV_ERR_CUDA; }
+            res->keep[size_t(c0 + j)] = std::shared_ptr<void>(h, [](void* q) { rv_host_free(q); });  // slot per chunk: rv_encoded_export(i) holds keep[i]
+            c.host = h;
+            GRP_CUDA(cudaMemcpyAsync(h, d_out[size_t(j)].p, bytes, cudaMemcpyDeviceToHost, stream));
+        }
+        ev.rec(7, stream);
+        GRP_CUDA(cudaStreamSynchronize(stream));
+        record_times();
+        return RV_OK;
+    }
+
+    // ---- outputs: the group's container blocks back to back in one device segment, framed there, then one D2H to `dst`
+    // (the group's place in the pinned file).  Block j's datums start after its count and size varints. ----
+    rv_status write_blocks(uint8_t* dst, const SyncMarker& sync) {
+        const int64_t seg = file_bytes();
+        GRP_CUDA(d_seg.alloc(size_t(seg)));
+        h_data.assign(static_cast<size_t>(k), nullptr);
+        int64_t off = 0;
+        for (int j = 0; j < k; ++j) {
+            const int64_t size = int64_t(chunk_tot[size_t(j)]);
+            const int64_t head = zz_len(rows_of(j)) + zz_len(size);
+            h_data[size_t(j)] = static_cast<uint8_t*>(d_seg.p) + off + head;
+            off += head + size + 16;
+        }
+        GRP_CUDA(d_ptrs.alloc(size_t(k) * 8));
+        GRP_CUDA(cudaMemcpyAsync(d_ptrs.p, h_data.data(), size_t(k) * 8, cudaMemcpyHostToDevice, stream));
+        p.out_data = static_cast<uint8_t* const*>(d_ptrs.p);
+        p.out_offsets = nullptr;
+        const rv_status st = launch_write<EO_OCF>();
+        if (st) return st;
+        ocf_frame_kernel<<<unsigned((k + 255) / 256), 256, 0, stream>>>(p, static_cast<const unsigned long long*>(d_tot.p), sync);
         ev.rec(5, stream);
         GRP_CUDA(cudaGetLastError());
+        ev.rec(6, stream);
+        GRP_CUDA(cudaMemcpyAsync(dst, d_seg.p, size_t(seg), cudaMemcpyDeviceToHost, stream));
+        ev.rec(7, stream);
+        GRP_CUDA(cudaStreamSynchronize(stream));
+        record_times();
+        return RV_OK;
     }
-    ev.rec(6, stream);
-    for (int j = 0; j < k; ++j) {
-        auto& c = res->chunks[size_t(c0 + j)];
-        const size_t bytes = off_bytes[size_t(j)] + size_t(c.data_bytes);
-        void* h = rv_host_alloc(bytes + 64);
-        if (!h) { *msg = "pinned allocation of an output chunk failed"; cudaStreamSynchronize(stream); return RV_ERR_CUDA; }
-        res->keep[size_t(c0 + j)] = std::shared_ptr<void>(h, [](void* q) { rv_host_free(q); });  // slot per chunk: rv_encoded_export(i) holds keep[i]
-        c.host = h;
-        GRP_CUDA(cudaMemcpyAsync(h, d_out[size_t(j)].p, bytes, cudaMemcpyDeviceToHost, stream));
-    }
-    ev.rec(7, stream);
-    GRP_CUDA(cudaStreamSynchronize(stream));
-    ms5[3] = ev.ms(0, 1);
-    ms5[4] = ev.ms(6, 7);
-    if (n > 0) { ms5[0] = ev.ms(1, 2); ms5[1] = ev.ms(2, 3); ms5[2] = ev.ms(4, 5); }
-    return RV_OK;
 #undef GRP_CUDA
+};
+
+// A schema every datum of which is empty: records of null fields only, at any depth.
+static bool always_empty(const AvroNode& s) {
+    if (s.k == AK::Null) return true;
+    if (s.k != AK::Record) return false;
+    for (const auto& f : s.fields)
+        if (!always_empty(*f.type)) return false;
+    return true;
 }
 
-rv_status rv_encode_host(const rv_schema* s, struct ArrowArray* batch, struct ArrowSchema* batch_schema, int64_t num_chunks, rv_encoded** out) {
-    if (!s || !batch || !batch_schema || !out) { rv_set_last_error("null argument"); return RV_ERR_INVALID; }
-    *out = nullptr;
-    struct Releaser {  // ownership of the C structs moved to us
-        ArrowArray* a; ArrowSchema* s;
-        ~Releaser() { if (a && a->release) a->release(a); if (s && s->release) s->release(s); }
-    } releaser{batch, batch_schema};
+struct Releaser {  // ownership of the C structs moved to us
+    ArrowArray* a; ArrowSchema* s;
+    ~Releaser() { if (a && a->release) a->release(a); if (s && s->release) s->release(s); }
+};
+
+// An Object Container File encode: rows per block, the sync marker and the file header up to and including it.
+struct OcfSpec {
+    int64_t block_records;
+    SyncMarker sync;
+    std::string header;
+};
+
+// Runs fn(g) for every group, each on its own host thread (group 0 on the caller's; a group that gets no thread runs on
+// the caller's too), and returns when all have finished.
+static void for_each_group(int groups, const std::function<void(int)>& fn) {
+    if (groups <= 1) { if (groups == 1) fn(0); return; }
+    std::vector<std::thread> pool;
+    for (int g = 1; g < groups; ++g) {
+        try { pool.emplace_back(fn, g); }
+        catch (const std::system_error&) { fn(g); }
+    }
+    fn(0);
+    for (auto& t : pool) t.join();
+}
+
+// The encode behind rv_encode_host, rv_encode_host_confluent (out = EO_CONFLUENT) and rv_encode_ocf_host (ocf != null: the
+// chunks are the file's blocks).
+static rv_status encode_batch(const rv_schema* s, const ArrowArray* batch, const ArrowSchema* batch_schema, int64_t num_chunks, int out_kind,
+                              uint32_t schema_id, const OcfSpec* ocf, rv_encoded** out) {
     if (rv_schema_is_projection(s)) {
         rv_set_last_error("fast_encode: a column projection (rv_schema_project) or a resolved handle (rv_schema_resolve) is not a schema to write with; encode with the full schema handle");
         return RV_ERR_INVALID;
     }
     if (!rv_schema_is_supported(s)) { rv_set_last_error("schema is outside the direct-encode subset; this library has no Value-tree CPU fallback"); return RV_ERR_SCHEMA; }
     const AvroNode* top = static_cast<const AvroNode*>(rv_schema_avro_root(s));
+    if (ocf && always_empty(*top)) {
+        rv_set_last_error("Object Container File: every datum of this schema is empty (records of null fields only), and a container block "
+                          "holds at most as many records as bytes, so no reader takes its blocks");
+        return RV_ERR_SCHEMA;
+    }
     if (std::strcmp(batch_schema->format, "+s") != 0) { rv_set_last_error("fast_encode: expected StructArray"); return RV_ERR_INVALID; }
     for (float& t : t_enc_timings) t = 0;
     {   // plan errors (missing column, wrong Arrow type, ...) surface before any GPU work, on the calling thread
@@ -813,48 +994,91 @@ rv_status rv_encode_host(const rv_schema* s, struct ArrowArray* batch, struct Ar
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) { rv_set_last_error("no CUDA device available (this library has no CPU fallback)"); return RV_ERR_CUDA; }
     ENC_CUDA(cudaGetDevice(&device));
     const int64_t n = batch->length;
-    const int64_t k64 = clamp_chunks(num_chunks, n);  // serialize.rs:15-17
+    int64_t k64, chunk_rows;
+    if (ocf) {  // block j = rows [j R, min((j + 1) R, n)): chunks of R rows, the last one takes the rest
+        chunk_rows = ocf->block_records;
+        k64 = n == 0 ? 0 : (n - 1) / chunk_rows + 1;
+    } else {
+        k64 = clamp_chunks(num_chunks, n);  // serialize.rs:15-17
+        chunk_rows = n / k64;               // slice_struct :19-30
+    }
+    if (k64 > int64_t(0x7FFFFFFF)) { rv_set_last_error("more than 2^31 - 1 blocks"); return RV_ERR_INVALID; }
     const int k = int(k64);
-    const int64_t chunk_rows = n / k;                 // slice_struct :19-30
     auto res = std::make_unique<rv_encoded>();
-    res->chunks.resize(size_t(k));
-    res->keep.resize(size_t(k));
-    for (int j = 0; j < k; ++j) res->chunks[size_t(j)].rows = (j == k - 1) ? n - chunk_rows * (k - 1) : chunk_rows;
+    if (!ocf) {
+        res->chunks.resize(size_t(k));
+        res->keep.resize(size_t(k));
+        for (int j = 0; j < k; ++j) res->chunks[size_t(j)].rows = (j == k - 1) ? n - chunk_rows * (k - 1) : chunk_rows;
+    }
 
     // Row groups of whole chunks, each on its own stream and host thread: the upload of group g+1 overlaps the kernels
     // and the download of group g (full-duplex PCIe), like the decode side's chunk pipeline.  Small batches: one group.
     int groups = 1;
     if (k >= 2 && n >= (int64_t(1) << 18)) groups = std::min(k, 4);
     if (const char* e = std::getenv("RV_ENC_GROUPS")) groups = std::max(1, std::min(k, std::atoi(e)));
+    if (k == 0) groups = 0;  // a container of no rows: the header alone, it ends after the header's sync marker
     std::vector<rv_status> status(size_t(groups), RV_OK);
     std::vector<std::string> message(static_cast<size_t>(groups));
     std::vector<std::array<float, 5>> times(static_cast<size_t>(groups), std::array<float, 5>{0, 0, 0, 0, 0});
-    auto run = [&](int g) {
-        cudaSetDevice(device);
+    std::vector<cudaStream_t> streams(static_cast<size_t>(groups), nullptr);
+    std::vector<std::unique_ptr<EncGroup>> grp(static_cast<size_t>(groups));
+    for (int g = 0; g < groups; ++g) {
         const int c0 = int(int64_t(g) * k / groups), c1 = int(int64_t(g + 1) * k / groups);
         const int64_t g0 = int64_t(c0) * chunk_rows, g1 = (c1 == k) ? n : int64_t(c1) * chunk_rows;
-        cudaStream_t stream = nullptr;
-        if (groups > 1 && cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking) != cudaSuccess) { status[size_t(g)] = RV_ERR_CUDA; message[size_t(g)] = "stream creation failed"; return; }
+        if (groups > 1 && cudaStreamCreateWithFlags(&streams[size_t(g)], cudaStreamNonBlocking) != cudaSuccess) {
+            status[size_t(g)] = RV_ERR_CUDA; message[size_t(g)] = "stream creation failed"; streams[size_t(g)] = nullptr;
+        }
+        grp[size_t(g)] = std::make_unique<EncGroup>(top, batch, batch_schema, g0, g1, c0, c1, chunk_rows, out_kind, schema_id, streams[size_t(g)],
+                                                    times[size_t(g)].data(), &message[size_t(g)]);
+    }
+    // one phase of group g on the group's host thread; bad_alloc there must not terminate the process
+    auto phase = [&](int g, rv_status (*step)(EncGroup&, void*), void* arg) {
+        if (status[size_t(g)] != RV_OK) return;
+        cudaSetDevice(device);
         try {
-            status[size_t(g)] = encode_group(top, batch, batch_schema, g0, g1, c0, c1, chunk_rows, stream, res.get(), times[size_t(g)].data(), &message[size_t(g)]);
-        } catch (const std::exception& e) {  // bad_alloc on a group's own thread must not terminate the process
-            cudaStreamSynchronize(stream);
+            status[size_t(g)] = step(*grp[size_t(g)], arg);
+        } catch (const std::exception& e) {
+            cudaStreamSynchronize(streams[size_t(g)]);
             (void)cudaGetLastError();
             status[size_t(g)] = RV_ERR_INVALID;
             message[size_t(g)] = e.what();
         }
-        if (stream) cudaStreamDestroy(stream);
     };
-    if (groups == 1) run(0);
-    else {
-        std::vector<std::thread> pool;
-        for (int g = 1; g < groups; ++g) {
-            try { pool.emplace_back(run, g); }
-            catch (const std::system_error&) { run(g); }   // no thread to be had: this group runs here
+    if (!ocf) {
+        for_each_group(groups, [&](int g) {
+            phase(g, [](EncGroup& e, void* r) { const rv_status st = e.measure(); return st ? st : e.write_chunks(static_cast<rv_encoded*>(r)); }, res.get());
+        });
+    } else {
+        // Two phases with a host barrier between them: a group's place in the file depends on the sizes of the groups
+        // before it, and the pinned file is allocated once, at its full size.
+        for_each_group(groups, [&](int g) { phase(g, [](EncGroup& e, void*) { return e.measure(); }, nullptr); });
+        bool ok = true;
+        for (int g = 0; g < groups; ++g) ok = ok && status[size_t(g)] == RV_OK;
+        if (ok) {  // (also with no groups: a file of no rows)
+            std::vector<int64_t> base(size_t(groups) + 1, int64_t(ocf->header.size()));
+            for (int g = 0; g < groups; ++g) base[size_t(g) + 1] = base[size_t(g)] + grp[size_t(g)]->file_bytes();
+            const int64_t len = base[size_t(groups)];
+            uint8_t* file = static_cast<uint8_t*>(rv_host_alloc(size_t(len)));
+            if (!file && groups == 0) { rv_set_last_error("pinned allocation of the container file failed"); return RV_ERR_CUDA; }
+            if (!file) {
+                status[0] = RV_ERR_CUDA;
+                message[0] = "pinned allocation of the container file failed";
+            } else {
+                res->keep.push_back(std::shared_ptr<void>(file, [](void* q) { rv_host_free(q); }));
+                res->file = file;
+                res->file_len = len;
+                std::memcpy(file, ocf->header.data(), ocf->header.size());
+                struct Dst { uint8_t* file; const int64_t* base; const SyncMarker* sync; int g; };
+                for_each_group(groups, [&](int g) {
+                    Dst d{file, base.data(), &ocf->sync, g};
+                    phase(g, [](EncGroup& e, void* a) { const Dst& d = *static_cast<Dst*>(a); return e.write_blocks(d.file + d.base[d.g], *d.sync); }, &d);
+                });
+            }
         }
-        run(0);
-        for (auto& t : pool) t.join();
     }
+    grp.clear();
+    for (cudaStream_t st : streams)
+        if (st) cudaStreamDestroy(st);
     for (int g = 0; g < groups; ++g) {
         if (status[size_t(g)] != RV_OK) { rv_set_last_error(message[size_t(g)].c_str()); return status[size_t(g)]; }  // lowest rows first
         for (int q = 0; q < 5; ++q) t_enc_timings[q] += times[size_t(g)][size_t(q)];
@@ -863,7 +1087,77 @@ rv_status rv_encode_host(const rv_schema* s, struct ArrowArray* batch, struct Ar
     return RV_OK;
 }
 
+extern "C" {
+
+rv_status rv_encode_host(const rv_schema* s, struct ArrowArray* batch, struct ArrowSchema* batch_schema, int64_t num_chunks, rv_encoded** out) {
+    if (!s || !batch || !batch_schema || !out) { rv_set_last_error("null argument"); return RV_ERR_INVALID; }
+    *out = nullptr;
+    Releaser releaser{batch, batch_schema};
+    return encode_batch(s, batch, batch_schema, num_chunks, EO_BINARY, 0, nullptr, out);
+}
+
+rv_status rv_encode_host_confluent(const rv_schema* s, struct ArrowArray* batch, struct ArrowSchema* batch_schema, int64_t num_chunks,
+                                   int64_t schema_id, rv_encoded** out) {
+    if (!s || !batch || !batch_schema || !out) { rv_set_last_error("null argument"); return RV_ERR_INVALID; }
+    *out = nullptr;
+    Releaser releaser{batch, batch_schema};
+    if (schema_id < 0 || schema_id > int64_t(0xFFFFFFFF)) {
+        rv_set_last_error(("Confluent schema id " + std::to_string(schema_id) + " is outside [0, 2^32 - 1]").c_str());
+        return RV_ERR_INVALID;
+    }
+    return encode_batch(s, batch, batch_schema, num_chunks, EO_CONFLUENT, uint32_t(schema_id), nullptr, out);
+}
+
+rv_status rv_encode_ocf_host(const rv_schema* s, struct ArrowArray* batch, struct ArrowSchema* batch_schema, int64_t block_records,
+                             const uint8_t* sync, const char* const* meta_keys, const uint8_t* const* meta_values,
+                             const int64_t* meta_value_lens, int64_t n_meta, rv_encoded** out) {
+    if (!s || !batch || !batch_schema || !out) { rv_set_last_error("null argument"); return RV_ERR_INVALID; }
+    *out = nullptr;
+    Releaser releaser{batch, batch_schema};
+    auto invalid = [](const std::string& m) { rv_set_last_error(("Object Container File: " + m).c_str()); return RV_ERR_INVALID; };
+    if (block_records < 1) return invalid("block_records must be at least 1, got " + std::to_string(block_records));
+    if (!sync) return invalid("the sync marker is null");
+    if (n_meta < 0) return invalid("n_meta must not be negative");
+    if (n_meta > 0 && (!meta_keys || !meta_values || !meta_value_lens)) return invalid("null metadata arrays");
+    OcfSpec ocf;
+    ocf.block_records = block_records;
+    std::memcpy(ocf.sync.b, sync, 16);
+    size_t json_len = 0;
+    const char* json = rv_internal_schema_json(s, &json_len);
+    std::string& h = ocf.header;
+    h.assign("Obj\x01", 4);
+    put_zz(h, 2 + n_meta);  // one metadata map block
+    put_zz(h, 11); h += "avro.schema"; put_zz(h, int64_t(json_len)); h.append(json ? json : "", json_len);
+    put_zz(h, 10); h += "avro.codec"; put_zz(h, 4); h += "null";
+    std::vector<std::string> seen;
+    for (int64_t i = 0; i < n_meta; ++i) {
+        const char* key = meta_keys[i];
+        const std::string at = "metadata entry " + std::to_string(i);
+        if (!key || !*key) return invalid(at + ": the key is empty");
+        const std::string kstr(key);
+        if (kstr.compare(0, 5, "avro.") == 0) return invalid(at + ": the key '" + kstr + "' is reserved (avro.*)");
+        if (std::find(seen.begin(), seen.end(), kstr) != seen.end()) return invalid(at + ": the key '" + kstr + "' repeats");
+        seen.push_back(kstr);
+        if (meta_value_lens[i] < 0) return invalid(at + ": negative value length");
+        if (meta_value_lens[i] > 0 && !meta_values[i]) return invalid(at + ": null value");
+        put_zz(h, int64_t(kstr.size())); h += kstr;
+        put_zz(h, meta_value_lens[i]);
+        if (meta_value_lens[i] > 0) h.append(reinterpret_cast<const char*>(meta_values[i]), size_t(meta_value_lens[i]));
+    }
+    put_zz(h, 0);
+    h.append(reinterpret_cast<const char*>(sync), 16);
+    return encode_batch(s, batch, batch_schema, 0, EO_OCF, 0, &ocf, out);
+}
+
 int64_t rv_encoded_num_chunks(const rv_encoded* r) { return r ? int64_t(r->chunks.size()) : 0; }
+
+rv_status rv_encoded_file(const rv_encoded* r, const uint8_t** data, int64_t* len) {
+    if (!r || !data || !len) { rv_set_last_error("null argument"); return RV_ERR_INVALID; }
+    if (!r->file) { rv_set_last_error("not an Object Container File result (rv_encode_ocf_host); export its chunks with rv_encoded_export"); return RV_ERR_INVALID; }
+    *data = r->file;
+    *len = r->file_len;
+    return RV_OK;
+}
 
 // Exports chunk i as an Arrow Binary array (format "z": i32 offsets + bytes), like GenericBinaryArray<i32>.
 rv_status rv_encoded_export(rv_encoded* r, int64_t i, struct ArrowArray* out_array, struct ArrowSchema* out_schema) {

@@ -405,6 +405,7 @@ static SchemaStats stats_at(const SchemaStats& st, int tile, const Plan& plan) {
 struct rv_schema {
     std::atomic<int> refs{1};
     std::shared_ptr<const AvroNode> avro;  // (shared with the handles projected from this one)
+    std::string json;             // the document rv_schema_parse parsed (a container file's avro.schema when encoding one)
     bool supported = false;
     std::string why;              // why it is unsupported / why no plan
     std::vector<ArrowField> fields;  // the columns of the batches, in their order
@@ -1072,6 +1073,7 @@ rv_status rv_schema_parse(const char* json, size_t len, rv_schema** out) {
     try {
         auto s = std::make_unique<rv_schema>();
         s->avro = parse_avro_schema(json, len);
+        s->json.assign(json, len);
         s->supported = is_supported(*s->avro, &s->why);
         if (s->avro->k == AK::Record) {
             try {
@@ -1882,6 +1884,10 @@ rv_status rv_dev_concat_bits(uint32_t* d_dst_words, int64_t dst_bit, const uint3
 void* rv_internal_dev_get(size_t bytes, int device, size_t* actual) { return devmem().get(bytes, device, actual); }
 void rv_internal_dev_put(void* p, size_t actual, int device) { devmem().put(p, actual, device); }
 const void* rv_schema_avro_root(const rv_schema* s) { return s ? s->avro.get() : nullptr; }
+const char* rv_internal_schema_json(const rv_schema* s, size_t* len) {
+    *len = s ? s->json.size() : 0;
+    return s ? s->json.data() : nullptr;
+}
 int rv_schema_is_projection(const rv_schema* s) { return s && (!s->keep.empty() || s->res) ? 1 : 0; }  // (or a resolution)
 void rv_set_last_error(const char* msg) { t_error = msg ? msg : ""; }
 
