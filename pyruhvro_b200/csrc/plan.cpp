@@ -4,6 +4,7 @@
 #include "plan.hpp"
 
 #include <algorithm>
+#include <cmath>
 #include <cstring>
 #include <stdexcept>
 
@@ -514,7 +515,16 @@ struct Builder {
             p.arrays[size_t(arr)].slot_v = sv;
         }
         uint64_t bits = 0;
-        if (out == NK_F32) { const float x = float(rs.def.d); uint32_t u; std::memcpy(&u, &x, 4); bits = u; }
+        if (out == NK_F32) {
+            // the default's double rounded to float once more, as Avro libraries that parse JSON numbers as doubles do.
+            // At or beyond FLT_MAX + half an ulp (2^128 - 2^103) the nearest float is infinity; float() of such a double
+            // is undefined in C++, so that case is spelled out.
+            const double d = rs.def.d;
+            const float x = std::fabs(d) >= 0x1.ffffffp127 ? (d < 0 ? -HUGE_VALF : HUGE_VALF) : float(d);
+            uint32_t u;
+            std::memcpy(&u, &x, 4);
+            bits = u;
+        }
         else if (out == NK_F64) std::memcpy(&bits, &rs.def.d, 8);
         else bits = uint64_t(rs.def.i);
         p.nodes[size_t(id)].aux = int32_t(uint32_t(bits));

@@ -4,6 +4,7 @@
 #include <algorithm>
 #include <cerrno>
 #include <climits>
+#include <cmath>
 #include <cstdint>
 #include <cstdlib>
 #include <cstring>
@@ -707,8 +708,12 @@ DefaultValue default_of(const AvroNode& t, const Json* j, const std::string& pat
         case AK::Float: case AK::Double: {
             if (j->kind != Json::Number) mismatch();
             char* end = nullptr;
+            errno = 0;
             d.d = std::strtod(j->str.c_str(), &end);
             if (!end || *end) mismatch();
+            // A number beyond the double range (1e400) is not a JSON number other Avro libraries read: serde_json refuses
+            // it.  Underflow (1e-400 -> 0, 5e-325 -> a subnormal) is accepted, as there.
+            if (errno == ERANGE && std::isinf(d.d)) mismatch();
             break;
         }
         case AK::String:

@@ -5,7 +5,6 @@ plan and walkers through the host emulation (tests/emu/resolve.py); tests/test_g
 import json
 import random
 
-import numpy as np
 import pytest
 
 import pyruhvro_b200 as pr
@@ -288,17 +287,21 @@ def test_kafka_v2_values(coracle):
 
 
 def test_promotions_round_once(coracle):
-    """long -> float / double with one rounding step: values just above a float's halfway point."""
+    """long -> float / double and int -> float with one rounding step, to nearest even, against the exact reference:
+    values just above a float's halfway point, and the ends of both ranges."""
+    from tests import exact_numbers as X
     wj = rec(fld("a", "long"), fld("b", "long"), fld("c", "int"))
     rj = rec(fld("a", "float"), fld("b", "double"), fld("c", "float"))
     vals = [{"a": v, "b": v, "c": c} for v, c in [((1 << 60) + (1 << 36) + 1, 16777217), (2 ** 63 - 1, -(2 ** 31)), (-(2 ** 63), 2 ** 31 - 1),
                                                      ((1 << 53) + 1, 16777219), (0, 0)]]
     ws = po.parse_schema(wj)
     data, off = po.pack_records([po.encode_datum(ws, v) for v in vals])
-    got = R.decode(wj, rj, data, off, len(vals), 1, walker="gen")[0].to_pydict()
-    assert got["a"] == [float(np.array([v["a"]]).astype(np.float32)[0]) for v in vals]
-    assert got["b"] == [float(np.array([v["b"]]).astype(np.float64)[0]) for v in vals]
-    assert got["c"] == [float(np.array([v["c"]]).astype(np.float32)[0]) for v in vals]
+    got = R.decode(wj, rj, data, off, len(vals), 1, walker="gen")[0]
+    bits = {c: memoryview(got.column(c).buffers()[1]).cast(fmt).tolist()[:len(vals)] for c, fmt in (("a", "I"), ("b", "Q"), ("c", "I"))}
+    assert bits["a"] == [X.int_to_f32_bits(v["a"]) for v in vals]
+    assert bits["b"] == [X.int_to_f64_bits(v["b"]) for v in vals]
+    assert bits["c"] == [X.int_to_f32_bits(v["c"]) for v in vals]
+    assert bits["a"][0] == 0x5D800001   # a rounding through double would give 0x5D800000
 
 
 # ---- damaged inputs: the writer-schema decode's verdict --------------------------------------------------------------

@@ -40,15 +40,21 @@ def schemas():
     from tests.test_gpu_ocf import BIG_SCHEMA
     from tests.test_ocf import BOOL_STR_SCHEMA, ZW_SCHEMA
     out += [BIG_SCHEMA, BOOL_STR_SCHEMA, ZW_SCHEMA]
+    from tests.test_resolve_edges import JIT_RESOLVED
+    out += JIT_RESOLVED  # a resolved plan (writer, reader) has its own walker
     return list(dict.fromkeys(out))
 
 
 def one(item):
-    """A schema, or (schema, columns) for a projected plan."""
+    """A schema, (schema, columns) for a projected plan or (writer, reader) for a resolved one."""
     import pyruhvro_b200 as pr
     sj, cols = item if isinstance(item, tuple) else (item, None)
     s = pr.Schema(sj)
-    (s if cols is None else s.project(list(cols))).precompile("sm_90a")
+    if isinstance(cols, str):
+        s = s.read_as(cols)
+    elif cols is not None:
+        s = s.project(list(cols))
+    s.precompile("sm_90a")
     return 1
 
 
