@@ -170,6 +170,44 @@ rv_status rv_decode_ocf_host_projected(const uint8_t* file, int64_t len, int64_t
 rv_status rv_decode_ocf_host_resolved(const uint8_t* file, int64_t len, int64_t num_chunks, const rv_schema* reader,
                                       const char* const* columns, int64_t n_columns, rv_schema** schema_out, rv_result** out);
 
+/* ---- several writer schemas: Confluent messages of a topic written with different schema versions ------------------
+ * A registry: the reader's schema and, for each registered schema id, the writer's schema it names.  Immutable and
+ * thread-safe once created; it keeps one resolved handle (rv_schema_resolve, projected to `columns` when given) per
+ * writer, so each writer's capacity history and compiled walker persist across calls, and a walker is compiled only when
+ * its id first appears in a call.
+ * columns: the reader's top-level fields the batches hold (rv_schema_project; NULL with n_columns 0: all of them).
+ * At most 256 writers.  Fails before any CUDA call:
+ *   RV_ERR_INVALID: no writers, more than 256, an id outside [0, 2^32 - 1] or registered twice, a projected or resolved
+ *                   handle as reader or writer, an unknown column;
+ *   RV_ERR_SCHEMA:  a writer that does not resolve to the reader ("schema id X: " then rv_schema_resolve's message). */
+typedef struct rv_versions rv_versions;
+rv_status rv_versions_create(const rv_schema* reader, const int64_t* schema_ids, const rv_schema* const* writers,
+                             int64_t n_writers, const char* const* columns, int64_t n_columns, rv_versions** out);
+void rv_versions_release(rv_versions* v);
+
+/* n Confluent messages (0x00, the big-endian u32 schema id, the datum) -> num_chunks batches in the reader's Arrow form
+ * (rv_schema_export_arrow of the reader, projected to the registry's columns), rows in message order.  Chunking is
+ * rv_decode_host's; row j of batch i is message i * floor(n / k) + j decoded with the writer schema its id names and
+ * resolved to the reader.  Batch i equals, buffer for buffer, the reader's decode of those messages each resolved and
+ * re-encoded with the reader's schema.
+ * Errors: the lowest failing message wins across every category, "(record N)" with N its index in the call.
+ *   RV_ERR_FRAME: a message shorter than 5 bytes or with a wrong magic byte, or whose id is not registered ("schema id
+ *                 X is not registered");
+ *   otherwise the status the message's writer's resolved decode gives for it (RV_ERR_ENUM for an unmapped symbol);
+ *   RV_ERR_OVERFLOW: a column of an output batch exceeds Arrow's i32 offsets.
+ * The messages are partitioned on the GPU into one group per (batch, writer), each group is decoded with its writer's
+ * resolved handle, and a take interleaves the groups' rows back into message order.  When every message carries the
+ * same id the input is decoded directly with that writer's handle.  Inputs, alignment and result ownership are those of
+ * rv_decode_host / rv_decode_device. */
+rv_status rv_decode_host_versions(const rv_versions* v, const uint8_t* data, const int64_t* offsets, int64_t n,
+                                  int64_t num_chunks, rv_result** out);
+rv_status rv_decode_device_versions(const rv_versions* v, const uint8_t* d_data, const int64_t* d_offsets, int64_t n,
+                                    int64_t num_chunks, void* cuda_stream, rv_result** out);
+/* CUDA-event timings of the calling thread's last rv_decode_*_versions call, in milliseconds: [0] partition, [1] the
+ * groups' decodes (the whole decode on the single-id path), [2] take (0 on the single-id path), [3] all of it on the
+ * device.  Returns how many entries were written. */
+int rv_last_versions_timings(float* out_ms, int cap);
+
 /* Copies a device-resident result's buffers to pinned host memory (no-op if already there). */
 rv_status rv_result_to_host(rv_result* r);
 

@@ -31,7 +31,7 @@ from . import _build
 __all__ = [
     "deserialize_array", "deserialize_array_threaded", "deserialize_array_threaded_spawn",
     "serialize_record_batch", "serialize_record_batch_spawn", "lib", "Schema", "decode_packed", "deserialize_arrow_array",
-    "deserialize_confluent", "deserialize_ocf", "serialize_confluent", "serialize_ocf",
+    "deserialize_confluent", "deserialize_confluent_versions", "deserialize_ocf", "serialize_confluent", "serialize_ocf",
 ]
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
@@ -83,6 +83,12 @@ def _bind(L):
     L.rv_schema_project.argtypes = [vp, vp, i64, ctypes.POINTER(vp)]
     L.rv_schema_resolve.argtypes = [vp, vp, ctypes.POINTER(vp)]
     L.rv_decode_ocf_host_resolved.argtypes = [vp, i64, i64, vp, vp, i64, ctypes.POINTER(vp), ctypes.POINTER(vp)]
+    L.rv_versions_create.argtypes = [vp, vp, vp, i64, vp, i64, ctypes.POINTER(vp)]
+    L.rv_versions_release.argtypes = [vp]
+    L.rv_versions_release.restype = None
+    L.rv_decode_host_versions.argtypes = [vp, vp, vp, i64, i64, ctypes.POINTER(vp)]
+    L.rv_decode_device_versions.argtypes = [vp, vp, vp, i64, i64, vp, ctypes.POINTER(vp)]
+    L.rv_last_versions_timings.argtypes = [ctypes.POINTER(ctypes.c_float), ctypes.c_int]
     L.rv_result_to_host.argtypes = [vp]
     L.rv_result_num_batches.restype = i64
     L.rv_result_num_batches.argtypes = [vp]
@@ -338,6 +344,77 @@ def deserialize_confluent(list, schema, num_chunks=1, schema_id=None, *, columns
         raise OverflowError("can't convert negative int to unsigned")
     return _decode_list(list, schema, num_chunks, framing=(5, 1, -1 if schema_id is None else int(schema_id)), columns=columns,
                         reader_schema=reader_schema)
+
+
+class Versions:
+    """A registry of writer schemas by Confluent schema id, read as one reader schema (rv_versions_create): the handle
+    deserialize_confluent_versions decodes with.  `writer_schemas` is a dict[int, str]; `columns` optionally names the
+    reader's top-level fields the batches hold."""
+
+    def __init__(self, writer_schemas, reader_schema: str, columns=None):
+        if not isinstance(writer_schemas, dict):
+            raise TypeError("argument 'writer_schemas': expected a dict[int, str]")
+        items = sorted(writer_schemas.items())
+        for sid, sj in items:
+            if not isinstance(sid, int) or not isinstance(sj, str):
+                raise TypeError("argument 'writer_schemas': expected a dict[int, str]")
+        self.reader = _get_or_parse_schema(reader_schema, columns)   # the batches' schema
+        full = _get_or_parse_schema(reader_schema)
+        self._writers = [_get_or_parse_schema(sj) for _, sj in items]   # kept alive with the registry
+        n = len(items)
+        ids = (ctypes.c_int64 * max(n, 1))(*[max(min(sid, 2 ** 63 - 1), -(2 ** 63)) for sid, _ in items])
+        hs = (ctypes.c_void_p * max(n, 1))(*[w.handle for w in self._writers])
+        names, keep = _column_names(columns) if columns is not None else (None, [])
+        h = ctypes.c_void_p()
+        _check(lib.rv_versions_create(full.handle, ids, hs, n, names, len(keep), ctypes.byref(h)))
+        self.handle = h.value
+
+    def __del__(self):
+        h, self.handle = getattr(self, "handle", None), None
+        if h:
+            lib.rv_versions_release(h)
+
+
+_versions_cache = {}
+
+
+def _get_or_create_versions(writer_schemas, reader_schema, columns) -> Versions:
+    if not isinstance(writer_schemas, dict):
+        raise TypeError("argument 'writer_schemas': expected a dict[int, str]")
+    if not isinstance(reader_schema, str):
+        raise TypeError("argument 'reader_schema': expected str")
+    if columns is not None:
+        if isinstance(columns, (str, bytes)):
+            raise TypeError("argument 'columns': expected a list of field names, not a single string")
+        columns = tuple(columns)
+    key = (tuple(sorted(writer_schemas.items())), reader_schema, columns)
+    with _schema_lock:
+        v = _versions_cache.get(key)
+    if v is not None:
+        return v
+    v = Versions(writer_schemas, reader_schema, columns)
+    with _schema_lock:
+        return _versions_cache.setdefault(key, v)
+
+
+def deserialize_confluent_versions(list, writer_schemas, reader_schema, num_chunks=1, *, columns=None):  # noqa: A002
+    """list[bytes] of Confluent-framed Kafka messages written with several schema versions -> `num_chunks` RecordBatches
+    in `reader_schema`'s Arrow form, rows in message order.  `writer_schemas` maps every schema id that may occur to the
+    writer schema it names (dict[int, str]); each message is decoded with its own writer's schema and resolved to the
+    reader (rv_decode_host_versions).  An id outside the map is an error, like a short message or a wrong magic byte."""
+    if num_chunks < 0:
+        raise OverflowError("can't convert negative int to unsigned")
+    if not isinstance(list, type([])):
+        raise TypeError("argument 'list': expected a list of bytes")
+    v = _get_or_create_versions(writer_schemas, reader_schema, columns)
+    return _export_batches(_ext().decode_list_versions(v.handle, list, int(num_chunks)), v.reader)
+
+
+def last_versions_timings() -> dict:
+    """CUDA-event times (ms) of the calling thread's last deserialize_confluent_versions / rv_decode_*_versions call."""
+    buf = (ctypes.c_float * 4)()
+    lib.rv_last_versions_timings(buf, 4)
+    return dict(zip(("partition", "decodes", "take", "device"), buf))
 
 
 def deserialize_array(list, schema, *, columns=None, reader_schema=None):  # noqa: A002 - the reference names the parameter `list`

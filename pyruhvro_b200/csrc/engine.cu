@@ -38,6 +38,7 @@
 #include "plan.hpp"
 #include "result.hpp"
 #include "schema.hpp"
+#include "versions.hpp"
 
 using namespace rv;
 
@@ -670,7 +671,8 @@ int64_t max_tile_span(const int64_t* offsets, int64_t n, int64_t k, int tile) {
 
 // ---- the decode call ------------------------------------------------------------------------
 rv_status decode_on_device(rv_schema* s, const uint8_t* d_data, const int64_t* d_offsets, int64_t n, int64_t num_chunks,
-                           const InputHints& hints, cudaStream_t stream, int device, rv_result** out, int64_t record_base = 0) {
+                           const InputHints& hints, cudaStream_t stream, int device, rv_result** out, int64_t record_base = 0,
+                           unsigned long long* err_word_out = nullptr) {
     const Plan& plan = s->plan;
     const int S = int(plan.streams.size());
     const int Sx = std::max(S, 1);
@@ -971,7 +973,7 @@ rv_status decode_on_device(rv_schema* s, const uint8_t* d_data, const int64_t* d
                     j.status = std::string("launch of the compiled walker was rejected: ") + cudaGetErrorString(le);
                 }
                 RV_CUDA(cudaStreamSynchronize(stream));
-                return decode_on_device(s, d_data, d_offsets, n, num_chunks, hints, stream, device, out, record_base);
+                return decode_on_device(s, d_data, d_offsets, n, num_chunks, hints, stream, device, out, record_base, err_word_out);
             }
         } else {
             launch_fused(p, smem_bytes, stream);
@@ -992,6 +994,7 @@ rv_status decode_on_device(rv_schema* s, const uint8_t* d_data, const int64_t* d
         const unsigned long long err_word = hb_ctrl[CW_ERR];
         if (err_word != ~0ull) {
             const uint32_t code = uint32_t(err_word & 0xFF);
+            if (err_word_out) *err_word_out = err_word;
             return fail(status_of(code), std::string(err_text(code)) + " (record " + std::to_string(int64_t(err_word >> 8) + record_base) + ")");
         }
         std::memcpy(chunk_tot.data(), hb_ctrl + CW_CHUNK_TOT, chunk_tot.size() * 8);
@@ -1950,5 +1953,364 @@ rv_status rv_schema_precompile(const rv_schema* s, const char* arch) {
 }
 const char* rv_last_error(void) { return t_error.c_str(); }
 const char* rv_version(void) { return "pyruhvro_b200 0.2.0 (sm_90a)"; }
+
+}  // extern "C"
+
+
+// ---- several writer schemas in one call (versions.hpp, versions.cu, DESIGN.md §7) -------------------------------------
+struct rv_versions {
+    rv_schema* reader = nullptr;          // the batches' schema: the reader's, projected to the columns
+    std::vector<int64_t> ids;             // ascending
+    std::vector<rv_schema*> writers;      // the resolved (and projected) handle of ids[i]
+    std::vector<VersionPairing> pairs;    // writers[i]'s plan next to the reader's
+    ~rv_versions() {
+        rv_schema_release(reader);
+        for (rv_schema* w : writers) rv_schema_release(w);
+    }
+};
+
+namespace {
+
+thread_local float t_vtimings[4] = {0, 0, 0, 0};
+thread_local EventPool t_vevents;
+
+struct SubResults {  // the groups' one-chunk batches; their arenas go back to the cache with them
+    std::vector<rv_result*> r;
+    ~SubResults() { for (rv_result* x : r) rv_result_free(x); }
+};
+
+// The message index of row `row` of writer w's part of chunk j: the space-0 row map read back (error paths only).
+rv_status global_index(const unsigned long long* d_map0, int64_t chunk_start, int64_t chunk_len, int w, int64_t row, cudaStream_t stream,
+                       int64_t* out) {
+    std::vector<unsigned long long> m(static_cast<size_t>(chunk_len));
+    RV_CUDA(cudaMemcpyAsync(m.data(), d_map0 + chunk_start, size_t(chunk_len) * 8, cudaMemcpyDeviceToHost, stream));
+    RV_CUDA(cudaStreamSynchronize(stream));
+    const unsigned long long want = take_pack(uint32_t(w), uint64_t(row));
+    for (int64_t r = 0; r < chunk_len; ++r)
+        if (m[size_t(r)] == want) { *out = chunk_start + r; return RV_OK; }
+    return fail(RV_ERR_CUDA, "internal error: a group row has no message");
+}
+
+rv_status decode_versions(const rv_versions* v, const uint8_t* d_data, const int64_t* d_offsets, int64_t n, int64_t num_chunks,
+                          int64_t total_bytes, cudaStream_t stream, int device, rv_result** out) {
+    for (float& t : t_vtimings) t = 0;
+    if (n == 0) return decode_on_device(v->reader, nullptr, nullptr, 0, num_chunks, InputHints{}, stream, device, out);
+    const int W = int(v->ids.size());
+    const int64_t k64 = clamp_chunks(num_chunks, n);
+    if (k64 > (int64_t(1) << 24)) return fail(RV_ERR_INVALID, "num_chunks above 2^24 is not supported");
+    const int k = int(k64);
+    const int64_t chunk_rows = n / k, last_rows = n - chunk_rows * (k - 1);
+    const int64_t tpc = std::max<int64_t>(1, (chunk_rows + kTakeBlock - 1) / kTakeBlock);
+    const int64_t n_tiles = tpc * (k - 1) + (last_rows + kTakeBlock - 1) / kTakeBlock;
+    if (n_tiles > 0x7FFFFFF0ll || n >= (int64_t(1) << 40)) return fail(RV_ERR_INVALID, "too many records for one call");
+    const size_t G = size_t(k) * size_t(W);
+    cudaEvent_t* ev = nullptr;
+    RV_CUDA(t_vevents.get(device, &ev));
+
+    // ---- partition: count + scan, one read-back of the group sizes and the framing errors
+    size_t off = 0;
+    auto take_off = [&](size_t bytes) { const size_t o = off; off = align_up(off + bytes, 16); return o; };
+    const size_t o_ids = take_off(size_t(W) * 4), o_err = take_off(8 + G * 16), o_tot = o_err + 8, o_cnt = take_off(size_t(n_tiles) * W * 4),
+                 o_bytes = take_off(size_t(n_tiles) * W * 8), o_msgw = take_off(size_t(n) * 2), o_map0 = take_off(size_t(n) * 8),
+                 o_gdata = take_off(G * 8), o_goff = take_off(G * 8);
+    DevBuf d_part, d_gdata, d_goffs, d_take;
+    RV_CUDA(d_part.alloc(off, stream));
+    SyncOnExit guard{stream};  // declared after the cached device blocks: runs before they go back to the cache
+    uint8_t* dp = static_cast<uint8_t*>(d_part.p);
+    std::vector<uint32_t> ids32(v->ids.begin(), v->ids.end());
+    VersionsParams p{};
+    p.data = d_data; p.offsets = d_offsets; p.n = n; p.chunk_rows = chunk_rows;
+    p.k = k; p.tiles_per_chunk = int32_t(tpc); p.n_tiles = int32_t(n_tiles); p.n_ids = W;
+    p.ids = reinterpret_cast<const uint32_t*>(dp + o_ids);
+    p.err = reinterpret_cast<unsigned long long*>(dp + o_err);
+    p.group_tot = reinterpret_cast<unsigned long long*>(dp + o_tot);
+    p.tile_cnt = reinterpret_cast<uint32_t*>(dp + o_cnt);
+    p.tile_bytes = reinterpret_cast<unsigned long long*>(dp + o_bytes);
+    p.msg_w = reinterpret_cast<uint16_t*>(dp + o_msgw);
+    p.map0 = reinterpret_cast<unsigned long long*>(dp + o_map0);
+    p.gdata_off = reinterpret_cast<const unsigned long long*>(dp + o_gdata);
+    p.goff_base = reinterpret_cast<const unsigned long long*>(dp + o_goff);
+    RV_CUDA(cudaEventRecord(ev[0], stream));
+    RV_CUDA(cudaMemcpyAsync(dp + o_ids, ids32.data(), ids32.size() * 4, cudaMemcpyHostToDevice, stream));
+    RV_CUDA(cudaMemsetAsync(dp + o_err, 0xFF, 8, stream));
+    launch_versions_partition(p, stream);
+    RV_CUDA(cudaGetLastError());
+    std::vector<unsigned long long> back(1 + G * 2);
+    RV_CUDA(cudaMemcpyAsync(back.data(), dp + o_err, back.size() * 8, cudaMemcpyDeviceToHost, stream));  // the err word, then the totals at o_tot
+    RV_CUDA(cudaStreamSynchronize(stream));
+    unsigned long long best = back[0];
+    auto cnt = [&](size_t g) { return int64_t(back[1 + 2 * g]); };
+    auto bytes = [&](size_t g) { return int64_t(back[2 + 2 * g]); };
+
+    // ---- every message carries the same registered id: the writer's own decode of the input, no copy, no take
+    if (best == ~0ull) {
+        for (int w = 0; w < W; ++w) {
+            int64_t c = 0;
+            for (int j = 0; j < k; ++j) c += cnt(size_t(j) * W + w);
+            if (c != n) continue;
+            RV_CUDA(cudaEventRecord(ev[1], stream));
+            InputHints h;
+            h.framing = rv_framing{5, 1, v->ids[size_t(w)]};
+            h.total_bytes = total_bytes;
+            const rv_status st = decode_on_device(v->writers[size_t(w)], d_data, d_offsets, n, num_chunks, h, stream, device, out);
+            if (st) return st;
+            RV_CUDA(cudaEventRecord(ev[2], stream));
+            RV_CUDA(cudaEventSynchronize(ev[2]));
+            cudaEventElapsedTime(&t_vtimings[0], ev[0], ev[1]);
+            cudaEventElapsedTime(&t_vtimings[1], ev[1], ev[2]);
+            cudaEventElapsedTime(&t_vtimings[3], ev[0], ev[2]);
+            guard.armed = false;
+            return RV_OK;
+        }
+    }
+
+    // ---- place the groups (16-byte aligned, 64 readable bytes after each) and scatter the messages into them
+    std::vector<unsigned long long> gdata_off(G), goff_base(G);
+    size_t data_total = 0, off_total = 0;
+    for (size_t g = 0; g < G; ++g) {
+        gdata_off[g] = data_total;
+        goff_base[g] = off_total;
+        if (cnt(g) == 0) continue;
+        data_total = align_up(data_total + size_t(bytes(g)) + 64, 16);
+        off_total += align_up(size_t(cnt(g)) + 1, 2);  // every group's offsets 16-byte aligned
+    }
+    RV_CUDA(d_gdata.alloc(std::max<size_t>(data_total, 64), stream));
+    RV_CUDA(d_goffs.alloc(std::max<size_t>(off_total, 1) * 8, stream));
+    RV_CUDA(cudaMemcpyAsync(dp + o_gdata, gdata_off.data(), G * 8, cudaMemcpyHostToDevice, stream));
+    RV_CUDA(cudaMemcpyAsync(dp + o_goff, goff_base.data(), G * 8, cudaMemcpyHostToDevice, stream));
+    p.gdata = static_cast<uint8_t*>(d_gdata.p);
+    p.goffs = static_cast<int64_t*>(d_goffs.p);
+    launch_versions_scatter(p, stream);
+    RV_CUDA(cudaGetLastError());
+    RV_CUDA(cudaEventRecord(ev[1], stream));
+
+    // ---- every group through its writer's resolved decode; the lowest failing message of all wins
+    SubResults subs;
+    subs.r.assign(G, nullptr);
+    for (size_t g = 0; g < G; ++g) {
+        if (cnt(g) == 0) continue;
+        const int j = int(g / size_t(W)), w = int(g % size_t(W));
+        InputHints h;
+        h.framing = rv_framing{5, 1, v->ids[size_t(w)]};
+        h.total_bytes = bytes(g);
+        unsigned long long ew = ~0ull;
+        const rv_status st = decode_on_device(v->writers[size_t(w)], p.gdata + gdata_off[g], p.goffs + goff_base[g], cnt(g), 1, h, stream,
+                                              device, &subs.r[g], 0, &ew);
+        if (!st) continue;
+        if (ew == ~0ull) return st;  // not an error of a message
+        int64_t msg = 0;
+        const rv_status st2 = global_index(p.map0, int64_t(j) * chunk_rows, j == k - 1 ? last_rows : chunk_rows, w, int64_t(ew >> 8), stream, &msg);
+        if (st2) return st2;
+        best = std::min(best, (static_cast<unsigned long long>(msg) << 8) | (ew & 0xFF));
+    }
+    if (best != ~0ull) {
+        const uint32_t code = uint32_t(best & 0xFF);
+        const int64_t rec = int64_t(best >> 8);
+        if (code == E_FRAME_ID) {
+            int64_t a = 0;
+            uint8_t hdr[5] = {0, 0, 0, 0, 0};
+            RV_CUDA(cudaMemcpyAsync(&a, d_offsets + rec, 8, cudaMemcpyDeviceToHost, stream));
+            RV_CUDA(cudaStreamSynchronize(stream));
+            RV_CUDA(cudaMemcpyAsync(hdr, d_data + a, 5, cudaMemcpyDeviceToHost, stream));
+            RV_CUDA(cudaStreamSynchronize(stream));
+            const uint32_t id = (uint32_t(hdr[1]) << 24) | (uint32_t(hdr[2]) << 16) | (uint32_t(hdr[3]) << 8) | uint32_t(hdr[4]);
+            return fail(RV_ERR_FRAME, "framed message: schema id " + std::to_string(id) + " is not registered (record " + std::to_string(rec) + ")");
+        }
+        return fail(status_of(code), std::string(err_text(code)) + " (record " + std::to_string(rec) + ")");
+    }
+
+    // ---- the output batches' exact layout: sums over each chunk's groups
+    const Plan& rp = v->reader->plan;
+    const int S1 = std::max(int(rp.streams.size()), 1);
+    std::vector<std::vector<VersionPart>> parts(static_cast<size_t>(k), std::vector<VersionPart>(static_cast<size_t>(W)));
+    std::vector<unsigned long long> chunk_tot(size_t(k) * size_t(S1), 0ull);
+    for (int j = 0; j < k; ++j) {
+        for (int w = 0; w < W; ++w) {
+            const rv_result* r = subs.r[size_t(j) * W + w];
+            if (r) parts[size_t(j)][size_t(w)] = VersionPart{&r->chunks[0], static_cast<const uint8_t*>(r->arenas[0]->dev)};
+        }
+        versions_chunk_totals(rp, v->pairs, parts[size_t(j)], chunk_tot.data() + size_t(j) * size_t(S1));
+        for (int i = 0; i < S1; ++i)
+            if (chunk_tot[size_t(j) * size_t(S1) + size_t(i)] > 0x7FFFFFFFull)
+                return fail(RV_ERR_OVERFLOW, std::string(err_text(E_OVERFLOW)) + ": a column of batch " + std::to_string(j) + " exceeds 2^31 - 1");
+    }
+    Layout L = compute_layout(rp, n, k, chunk_tot.data());
+    auto arena_sp = std::make_shared<Arena>();
+    arena_sp->device = device;
+    arena_sp->bytes = L.total_bytes;
+    arena_sp->dev = devmem().get(std::max<size_t>(L.total_bytes, 64), device, &arena_sp->dev_actual);
+    if (!arena_sp->dev) return fail(RV_ERR_CUDA, "device allocation of the Arrow buffer arena failed (" + std::to_string(L.total_bytes) + " bytes)");
+    uint8_t* arena = static_cast<uint8_t*>(arena_sp->dev);
+
+    // ---- the take, one level of row spaces after the other
+    std::vector<const unsigned long long*> map0(static_cast<size_t>(k));
+    for (int j = 0; j < k; ++j) map0[size_t(j)] = p.map0 + int64_t(j) * chunk_rows;
+    const size_t take_bytes = plan_take(rp, v->pairs, parts, L.chunks, arena, map0, nullptr).total_bytes;
+    RV_CUDA(d_take.alloc(std::max<size_t>(take_bytes, 64), stream));
+    const TakePlan tp = plan_take(rp, v->pairs, parts, L.chunks, arena, map0, static_cast<uint8_t*>(d_take.p));
+    RV_CUDA(cudaEventRecord(ev[2], stream));
+    RV_CUDA(cudaMemcpyAsync(d_take.p, tp.header.data(), tp.header_bytes, cudaMemcpyHostToDevice, stream));
+    for (size_t l = 0; l + 1 < tp.level_first.size(); ++l)
+        launch_take_level(tp.spaces + tp.level_first[l], tp.level_first[l + 1] - tp.level_first[l], tp.level_blocks[l], tp.jobs,
+                          tp.scans + tp.scan_first[l], tp.scan_first[l + 1] - tp.scan_first[l], stream);
+    RV_CUDA(cudaGetLastError());
+    RV_CUDA(cudaEventRecord(ev[3], stream));
+    RV_CUDA(cudaStreamSynchronize(stream));
+    guard.armed = false;
+    cudaEventElapsedTime(&t_vtimings[0], ev[0], ev[1]);
+    cudaEventElapsedTime(&t_vtimings[1], ev[1], ev[2]);
+    cudaEventElapsedTime(&t_vtimings[2], ev[2], ev[3]);
+    cudaEventElapsedTime(&t_vtimings[3], ev[0], ev[3]);
+
+    auto res = std::make_unique<rv_result>();
+    res->schema = rv_schema_retain(v->reader);
+    for (int j = 0; j < k; ++j) versions_null_counts(rp, v->pairs, parts[size_t(j)], L.chunks[size_t(j)]);
+    res->chunks = std::move(L.chunks);
+    res->arenas.assign(res->chunks.size(), arena_sp);
+    res->arrow_bytes = exported_bytes(rp, res->chunks);
+    *out = res.release();
+    return RV_OK;
+}
+
+rv_status check_versions_input(const rv_versions* v, int64_t n, bool have_ptrs, rv_result** out) {
+    if (!out) return fail(RV_ERR_INVALID, "null argument");
+    *out = nullptr;
+    if (!v) return fail(RV_ERR_INVALID, "null versions handle");
+    if (n < 0 || (n > 0 && !have_ptrs)) return fail(RV_ERR_INVALID, "bad input pointers");
+    return RV_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+rv_status rv_versions_create(const rv_schema* reader, const int64_t* schema_ids, const rv_schema* const* writers, int64_t n_writers,
+                             const char* const* columns, int64_t n_columns, rv_versions** out) {
+    if (!out) return fail(RV_ERR_INVALID, "null argument");
+    *out = nullptr;
+    if (!reader || (n_writers > 0 && (!schema_ids || !writers)) || (!columns && n_columns != 0) || n_columns < 0)
+        return fail(RV_ERR_INVALID, "null argument");
+    if (n_writers < 1) return fail(RV_ERR_INVALID, "schema versions: no writer schemas");
+    if (n_writers > kMaxVersions) return fail(RV_ERR_INVALID, "schema versions: more than " + std::to_string(kMaxVersions) + " writer schemas");
+    auto bad_handle = [](const rv_schema* s) { return !s || !s->keep.empty() || s->res; };
+    if (bad_handle(reader)) return fail(RV_ERR_INVALID, "schema versions: pass the handle of the reader's full schema (rv_schema_parse)");
+    std::vector<size_t> order(static_cast<size_t>(n_writers));
+    for (int64_t i = 0; i < n_writers; ++i) {
+        order[size_t(i)] = size_t(i);
+        if (schema_ids[i] < 0 || schema_ids[i] > int64_t(0xFFFFFFFFu))
+            return fail(RV_ERR_INVALID, "schema versions: schema id " + std::to_string(schema_ids[i]) + " is not a u32");
+        if (bad_handle(writers[i]))
+            return fail(RV_ERR_INVALID, "schema versions: pass the handles of the writers' full schemas (rv_schema_parse), schema id " +
+                                            std::to_string(schema_ids[i]));
+    }
+    std::sort(order.begin(), order.end(), [&](size_t a, size_t b) { return schema_ids[a] < schema_ids[b]; });
+    for (size_t i = 1; i < order.size(); ++i)
+        if (schema_ids[order[i]] == schema_ids[order[i - 1]])
+            return fail(RV_ERR_INVALID, "schema versions: schema id " + std::to_string(schema_ids[order[i]]) + " is registered twice");
+    rv_status st = check_decodable(reader);
+    if (st) return st;
+    auto v = std::make_unique<rv_versions>();
+    if (columns) {
+        st = rv_schema_project(reader, columns, n_columns, &v->reader);
+        if (st) return st;
+    } else {
+        v->reader = rv_schema_retain(const_cast<rv_schema*>(reader));
+    }
+    for (size_t i : order) {
+        const std::string who = "schema id " + std::to_string(schema_ids[i]) + ": ";
+        rv_schema* r = nullptr;
+        st = rv_schema_resolve(writers[i], reader, &r);
+        if (st) return fail(st, who + t_error);
+        if (columns) {
+            rv_schema* full = r;
+            st = rv_schema_project(full, columns, n_columns, &r);
+            rv_schema_release(full);
+            if (st) return fail(st, who + t_error);
+        }
+        v->ids.push_back(schema_ids[i]);
+        v->writers.push_back(r);
+        try {
+            v->pairs.push_back(pair_plans(v->reader->plan, r->plan));
+        } catch (const std::exception& e) {
+            return fail(RV_ERR_SCHEMA, who + e.what());
+        }
+    }
+    *out = v.release();
+    return RV_OK;
+}
+
+void rv_versions_release(rv_versions* v) { delete v; }
+
+rv_status rv_decode_device_versions(const rv_versions* v, const uint8_t* d_data, const int64_t* d_offsets, int64_t n, int64_t num_chunks,
+                                    void* cuda_stream, rv_result** out) {
+    rv_status st = check_versions_input(v, n, d_data && d_offsets, out);
+    if (st) return st;
+    if (reinterpret_cast<uintptr_t>(d_data) & 15u) return fail(RV_ERR_INVALID, "d_data must be 16-byte aligned");
+    int device = 0;
+    st = ensure_cuda(&device);
+    if (st) return st;
+    cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
+    try {
+        st = decode_versions(v, d_data, d_offsets, n, num_chunks, -1, stream, device, out);
+    } catch (const std::exception& e) {
+        st = fail(RV_ERR_INVALID, e.what());
+    }
+    if (st) { const std::string keep = t_error; cudaStreamSynchronize(stream); (void)cudaGetLastError(); t_error = keep; }
+    return st;
+}
+
+rv_status rv_decode_host_versions(const rv_versions* v, const uint8_t* data, const int64_t* offsets, int64_t n, int64_t num_chunks,
+                                  rv_result** out) {
+    rv_status st = check_versions_input(v, n, data && offsets, out);
+    if (st) return st;
+    int device = 0;
+    st = ensure_cuda(&device);
+    if (st) return st;
+    cudaStream_t stream = nullptr;
+    DevBuf d_data, d_off;
+    const uint8_t* base = nullptr;
+    int64_t total = 0;
+    float h2d = 0, d2h = 0;
+    if (n > 0) {
+        const int64_t b0 = offsets[0];
+        total = offsets[n] - b0;
+        if (total < 0) return fail(RV_ERR_INVALID, "offsets are not monotonic");
+        RV_CUDA(d_data.alloc(size_t(total) + 64, stream));
+        RV_CUDA(d_off.alloc(size_t(n + 1) * 8, stream));
+        cudaEvent_t* ev = nullptr;
+        RV_CUDA(t_events.get(device, &ev));
+        RV_CUDA(cudaEventRecord(ev[4], stream));
+        // the caller's absolute offsets, with the base pointer biased so that base + offsets[i] addresses message i
+        cudaError_t e = upload(static_cast<uint8_t*>(d_data.p) + (b0 & 15), data + b0, size_t(total), device, stream);
+        if (e == cudaSuccess) e = upload(static_cast<uint8_t*>(d_off.p), reinterpret_cast<const uint8_t*>(offsets), size_t(n + 1) * 8, device, stream);
+        if (e == cudaSuccess) e = cudaEventRecord(ev[5], stream);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(stream);
+        if (e != cudaSuccess) { (void)cudaStreamSynchronize(stream); return fail(RV_ERR_CUDA, std::string("host->device copy: ") + cudaGetErrorString(e)); }
+        cudaEventElapsedTime(&h2d, ev[4], ev[5]);
+        base = static_cast<const uint8_t*>(d_data.p) + (b0 & 15) - b0;
+    }
+    try {
+        st = decode_versions(v, base, static_cast<const int64_t*>(d_off.p), n, num_chunks, total, stream, device, out);
+    } catch (const std::exception& e) {
+        st = fail(RV_ERR_INVALID, e.what());
+    }
+    if (st) { const std::string keep = t_error; cudaStreamSynchronize(stream); (void)cudaGetLastError(); t_error = keep; return st; }
+    const Arena* last = nullptr;
+    for (auto& a : (*out)->arenas) {
+        if (a.get() == last) continue;
+        last = a.get();
+        st = arena_to_host(**out, *a, stream, &d2h);
+        if (st) { rv_result_free(*out); *out = nullptr; return st; }
+    }
+    t_timings[4] = h2d;
+    t_timings[5] = d2h;
+    return RV_OK;
+}
+
+int rv_last_versions_timings(float* out_ms, int cap) {
+    const int n = cap < 4 ? cap : 4;
+    for (int i = 0; i < n; ++i) out_ms[i] = t_vtimings[i];
+    return n;
+}
 
 }  // extern "C"

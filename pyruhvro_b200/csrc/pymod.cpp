@@ -168,6 +168,41 @@ PyObject* decode_list(PyObject*, PyObject* args) {
     return PyLong_FromUnsignedLongLong(static_cast<unsigned long long>(reinterpret_cast<uintptr_t>(result)));
 }
 
+// decode_list_versions(versions_handle: int, records: list[bytes], num_chunks: int) -> result handle (int): Confluent
+// messages of several writer schemas (rv_decode_host_versions), through the same pinned gather as decode_list
+PyObject* decode_list_versions(PyObject*, PyObject* args) {
+    unsigned long long addr = 0;
+    PyObject* list = nullptr;
+    long long num_chunks = 1;
+    if (!PyArg_ParseTuple(args, "KO!L", &addr, &PyList_Type, &list, &num_chunks)) return nullptr;
+    const rv_versions* v = reinterpret_cast<const rv_versions*>(static_cast<uintptr_t>(addr));
+    PinnedPair slabs;
+    Packed pk;
+    bool first = true;
+    auto alloc = [&](size_t bytes) -> void* {
+        void* p = rv_host_alloc(bytes);
+        (first ? slabs.a : slabs.b) = p;
+        first = false;
+        return p;
+    };
+    try {
+        if (!pack_list(list, alloc, &pk)) return nullptr;
+    } catch (const std::exception& e) {
+        PyErr_SetString(PyExc_MemoryError, e.what());
+        return nullptr;
+    }
+    rv_result* result = nullptr;
+    rv_status st = RV_OK;
+    Py_BEGIN_ALLOW_THREADS;
+    st = rv_decode_host_versions(v, reinterpret_cast<const uint8_t*>(pk.data), pk.offsets, pk.n, num_chunks, &result);
+    Py_END_ALLOW_THREADS;
+    if (st != RV_OK) {
+        PyErr_SetString(PyExc_ValueError, rv_last_error());
+        return nullptr;
+    }
+    return PyLong_FromUnsignedLongLong(static_cast<unsigned long long>(reinterpret_cast<uintptr_t>(result)));
+}
+
 // pack(records: list[bytes]) -> (data: bytes, offsets: bytes of int64[n+1]).  The packing step alone, into ordinary
 // memory: lets the CPU test-suite check the list walk / gather without a GPU.
 PyObject* pack(PyObject*, PyObject* args) {
@@ -192,6 +227,7 @@ PyObject* pack(PyObject*, PyObject* args) {
 
 PyMethodDef methods[] = {
     {"decode_list", decode_list, METH_VARARGS, "decode_list(schema_handle, records: list[bytes], num_chunks[, header_bytes, check_magic, schema_id]) -> result handle"},
+    {"decode_list_versions", decode_list_versions, METH_VARARGS, "decode_list_versions(versions_handle, records: list[bytes], num_chunks) -> result handle"},
     {"pack", pack, METH_VARARGS, "pack(records: list[bytes]) -> (data, offsets): the packing step alone (test hook)"},
     {nullptr, nullptr, 0, nullptr},
 };
