@@ -50,7 +50,7 @@ typedef enum rv_status {
     RV_ERR_INVALID = 9,      /* bad argument */
     RV_ERR_CUDA = 10,        /* CUDA runtime failure (includes "no device") */
     RV_ERR_VALUE = 11,       /* wider subset: uuid text that is not a UUID, decimal wider than 128 bits */
-    RV_ERR_FRAME = 12        /* framed input: message shorter than its header, wrong magic byte, unexpected schema id */
+    RV_ERR_FRAME = 12        /* framed input: message shorter than its header, wrong magic byte, unexpected schema id or fingerprint */
 } rv_status;
 
 /* ---- schema --------------------------------------------------------------------------- */
@@ -107,6 +107,18 @@ rv_status rv_schema_project(const rv_schema* s, const char* const* columns, int6
  * passed as writer or reader. */
 rv_status rv_schema_resolve(const rv_schema* writer, const rv_schema* reader, rv_schema** out);
 
+/* The Avro specification's Parsing Canonical Form of the schema and its CRC-64-AVRO fingerprint (the 64-bit Rabin
+ * fingerprint, EMPTY = 0xc15d213aa4d7a795), the key single-object encoding names a writer schema by.  The form keeps
+ * primitives as bare names, named types by fullname (in full at their first occurrence, by fullname after that), only
+ * name / type / fields / symbols / items / values / size in that order, and drops namespaces, logical types, docs,
+ * aliases, defaults and whitespace.  Schemas that differ only in what is dropped share a fingerprint.
+ * For a projected or resolved handle both describe the writer's full schema: the schema the messages were written with.
+ * rv_schema_canonical_form returns the form's length and copies at most cap-1 bytes + NUL into buf (buf may be NULL).
+ * A schema with a construct the parser keeps as unsupported (duration, local-timestamp-*, timestamp-nanos, a recursive
+ * type, ...) has no form here: -1 / RV_ERR_SCHEMA. */
+int64_t rv_schema_canonical_form(const rv_schema* s, char* buf, size_t cap);
+rv_status rv_schema_fingerprint(const rv_schema* s, uint64_t* out);
+
 /* ---- decode ---------------------------------------------------------------------------- */
 
 /* Replaces ruhvro::deserialize::per_datum_deserialize_threaded (ruhvro/src/deserialize.rs:76-121)
@@ -149,6 +161,16 @@ rv_status rv_decode_host_framed(const rv_schema* s, const uint8_t* data, const i
 rv_status rv_decode_device_framed(const rv_schema* s, const uint8_t* d_data, const int64_t* d_offsets, int64_t n,
                                   int64_t num_chunks, const rv_framing* framing, void* cuda_stream, rv_result** out);
 
+/* Avro single-object encoding: every message is C3 01, the little-endian CRC-64-AVRO fingerprint of the writer's schema
+ * (rv_schema_fingerprint of `s`: the writer's, also for a projected or resolved handle), then the datum.  The header is
+ * checked and skipped inside the decode kernel.  A message shorter than 10 bytes, not starting with C3 01 or naming
+ * another fingerprint is RV_ERR_FRAME with its record index; the lowest failing record wins as on every path.
+ * RV_ERR_SCHEMA: a schema without a canonical form.  Otherwise rv_decode_host / rv_decode_device. */
+rv_status rv_decode_host_single_object(const rv_schema* s, const uint8_t* data, const int64_t* offsets, int64_t n,
+                                       int64_t num_chunks, rv_result** out);
+rv_status rv_decode_device_single_object(const rv_schema* s, const uint8_t* d_data, const int64_t* d_offsets, int64_t n,
+                                         int64_t num_chunks, void* cuda_stream, rv_result** out);
+
 /* An Avro Object Container File (magic, header with avro.schema / avro.codec, blocks of datums between sync markers;
  * uncompressed blocks only) -> `num_chunks` batches in pinned host memory.  The schema comes from the file: a new handle is
  * returned in *schema_out (release it with rv_schema_release).  Datums inside a block carry no lengths: the host walks
@@ -184,15 +206,24 @@ typedef struct rv_versions rv_versions;
 rv_status rv_versions_create(const rv_schema* reader, const int64_t* schema_ids, const rv_schema* const* writers,
                              int64_t n_writers, const char* const* columns, int64_t n_columns, rv_versions** out);
 void rv_versions_release(rv_versions* v);
+/* A registry of single-object writers, keyed by the fingerprints of writers[0 .. n_writers) (rv_schema_fingerprint).
+ * Everything else is rv_versions_create's.  Fails before any CUDA call, RV_ERR_INVALID: two writers with the same
+ * fingerprint (schemas that differ only in what the canonical form drops, which the wire cannot tell apart), no writers
+ * or more than 256, a projected or resolved handle, an unknown column.  RV_ERR_SCHEMA: a writer without a canonical form,
+ * a writer that does not resolve to the reader. */
+rv_status rv_versions_create_single_object(const rv_schema* reader, const rv_schema* const* writers, int64_t n_writers,
+                                           const char* const* columns, int64_t n_columns, rv_versions** out);
 
-/* n Confluent messages (0x00, the big-endian u32 schema id, the datum) -> num_chunks batches in the reader's Arrow form
+/* n Confluent messages (0x00, the big-endian u32 schema id, the datum) -- or, for a single-object registry, n
+ * single-object messages (C3 01, the writer's fingerprint, the datum) -- -> num_chunks batches in the reader's Arrow form
  * (rv_schema_export_arrow of the reader, projected to the registry's columns), rows in message order.  Chunking is
  * rv_decode_host's; row j of batch i is message i * floor(n / k) + j decoded with the writer schema its id names and
  * resolved to the reader.  Batch i equals, buffer for buffer, the reader's decode of those messages each resolved and
  * re-encoded with the reader's schema.
  * Errors: the lowest failing message wins across every category, "(record N)" with N its index in the call.
  *   RV_ERR_FRAME: a message shorter than 5 bytes or with a wrong magic byte, or whose id is not registered ("schema id
- *                 X is not registered");
+ *                 X is not registered"); single-object: shorter than 10 bytes, not C3 01, or a fingerprint that is not
+ *                 registered ("schema fingerprint 0x... is not registered");
  *   otherwise the status the message's writer's resolved decode gives for it (RV_ERR_ENUM for an unmapped symbol);
  *   RV_ERR_OVERFLOW: a column of an output batch exceeds Arrow's i32 offsets.
  * The messages are partitioned on the GPU into one group per (batch, writer), each group is decoded with its writer's
@@ -257,6 +288,12 @@ int rv_last_encode_timings(float* out_ms, int cap);
  * and the i32 overflow check of a chunk counts the headers.  schema_id outside [0, 2^32 - 1] is RV_ERR_INVALID. */
 rv_status rv_encode_host_confluent(const rv_schema* s, struct ArrowArray* batch, struct ArrowSchema* batch_schema,
                                    int64_t num_chunks, int64_t schema_id, rv_encoded** out);
+
+/* Avro single-object encoding: every datum is preceded by C3 01 and the little-endian CRC-64-AVRO fingerprint of `s`
+ * (rv_schema_fingerprint), 10 bytes.  Chunking and export are rv_encode_host_confluent's; the i32 overflow check of a
+ * chunk counts the headers.  RV_ERR_SCHEMA: a schema without a canonical form. */
+rv_status rv_encode_host_single_object(const rv_schema* s, struct ArrowArray* batch, struct ArrowSchema* batch_schema,
+                                       int64_t num_chunks, rv_encoded** out);
 
 /* One Object Container File of the batch's rows, codec "null":
  *   "Obj" 1, one metadata map block of 2 + n_meta entries: avro.schema (the exact text `s` was parsed from), avro.codec

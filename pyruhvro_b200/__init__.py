@@ -32,6 +32,7 @@ __all__ = [
     "deserialize_array", "deserialize_array_threaded", "deserialize_array_threaded_spawn",
     "serialize_record_batch", "serialize_record_batch_spawn", "lib", "Schema", "decode_packed", "deserialize_arrow_array",
     "deserialize_confluent", "deserialize_confluent_versions", "deserialize_ocf", "serialize_confluent", "serialize_ocf",
+    "deserialize_single_object", "deserialize_single_object_versions", "serialize_single_object",
 ]
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
@@ -78,12 +79,18 @@ def _bind(L):
     L.rv_decode_device.argtypes = [vp, vp, vp, i64, i64, vp, ctypes.POINTER(vp)]
     L.rv_decode_host_framed.argtypes = [vp, vp, vp, i64, i64, vp, ctypes.POINTER(vp)]
     L.rv_decode_device_framed.argtypes = [vp, vp, vp, i64, i64, vp, vp, ctypes.POINTER(vp)]
+    L.rv_decode_host_single_object.argtypes = [vp, vp, vp, i64, i64, ctypes.POINTER(vp)]
+    L.rv_decode_device_single_object.argtypes = [vp, vp, vp, i64, i64, vp, ctypes.POINTER(vp)]
+    L.rv_schema_canonical_form.restype = i64
+    L.rv_schema_canonical_form.argtypes = [vp, cp, ctypes.c_size_t]
+    L.rv_schema_fingerprint.argtypes = [vp, ctypes.POINTER(ctypes.c_uint64)]
     L.rv_decode_ocf_host.argtypes = [vp, i64, i64, ctypes.POINTER(vp), ctypes.POINTER(vp)]
     L.rv_decode_ocf_host_projected.argtypes = [vp, i64, i64, vp, i64, ctypes.POINTER(vp), ctypes.POINTER(vp)]
     L.rv_schema_project.argtypes = [vp, vp, i64, ctypes.POINTER(vp)]
     L.rv_schema_resolve.argtypes = [vp, vp, ctypes.POINTER(vp)]
     L.rv_decode_ocf_host_resolved.argtypes = [vp, i64, i64, vp, vp, i64, ctypes.POINTER(vp), ctypes.POINTER(vp)]
     L.rv_versions_create.argtypes = [vp, vp, vp, i64, vp, i64, ctypes.POINTER(vp)]
+    L.rv_versions_create_single_object.argtypes = [vp, vp, i64, vp, i64, ctypes.POINTER(vp)]
     L.rv_versions_release.argtypes = [vp]
     L.rv_versions_release.restype = None
     L.rv_decode_host_versions.argtypes = [vp, vp, vp, i64, i64, ctypes.POINTER(vp)]
@@ -104,6 +111,7 @@ def _bind(L):
     L.rv_result_free.restype = None
     L.rv_encode_host.argtypes = [vp, vp, vp, i64, ctypes.POINTER(vp)]
     L.rv_encode_host_confluent.argtypes = [vp, vp, vp, i64, i64, ctypes.POINTER(vp)]
+    L.rv_encode_host_single_object.argtypes = [vp, vp, vp, i64, ctypes.POINTER(vp)]
     L.rv_encode_ocf_host.argtypes = [vp, vp, vp, i64, vp, vp, vp, vp, i64, ctypes.POINTER(vp)]
     L.rv_encoded_file.argtypes = [vp, ctypes.POINTER(vp), ctypes.POINTER(i64)]
     L.rv_encoded_num_chunks.restype = i64
@@ -195,6 +203,24 @@ class Schema:
         h = ctypes.c_void_p()
         _check(lib.rv_schema_resolve(self.handle, reader.handle, ctypes.byref(h)))
         return Schema._adopt(h.value)
+
+    @property
+    def canonical_form(self) -> str:
+        """The Avro specification's Parsing Canonical Form of the writer's full schema (also for a projected or resolved
+        handle: the schema the data was written with)."""
+        n = lib.rv_schema_canonical_form(self.handle, None, 0)
+        if n < 0:
+            raise ValueError(_last_error())
+        buf = ctypes.create_string_buffer(n + 1)
+        lib.rv_schema_canonical_form(self.handle, buf, n + 1)
+        return buf.value.decode()
+
+    @property
+    def fingerprint(self) -> int:
+        """The CRC-64-AVRO fingerprint of canonical_form, as an unsigned int: the key single-object messages carry."""
+        fp = ctypes.c_uint64()
+        _check(lib.rv_schema_fingerprint(self.handle, ctypes.byref(fp)))
+        return fp.value
 
     @property
     def is_supported(self) -> bool:
@@ -346,12 +372,38 @@ def deserialize_confluent(list, schema, num_chunks=1, schema_id=None, *, columns
                         reader_schema=reader_schema)
 
 
-class Versions:
-    """A registry of writer schemas by Confluent schema id, read as one reader schema (rv_versions_create): the handle
-    deserialize_confluent_versions decodes with.  `writer_schemas` is a dict[int, str]; `columns` optionally names the
-    reader's top-level fields the batches hold."""
+def deserialize_single_object(list, schema, num_chunks=1, *, columns=None, reader_schema=None):  # noqa: A002
+    """list[bytes] of Avro single-object messages (C3 01 + the little-endian CRC-64-AVRO fingerprint of the writer schema
+    + Avro datum) -> `num_chunks` RecordBatches.  Every header must name `schema`'s fingerprint (Schema.fingerprint); it is
+    checked and skipped inside the decode kernel (rv_decode_host_single_object)."""
+    if num_chunks < 0:
+        raise OverflowError("can't convert negative int to unsigned")
+    if not isinstance(list, type([])):
+        raise TypeError("argument 'list': expected a list of bytes")
+    s = _get_or_parse_schema(schema, columns, reader_schema)
+    return _export_batches(_ext().decode_list_single_object(s.handle, list, int(num_chunks)), s)
 
-    def __init__(self, writer_schemas, reader_schema: str, columns=None):
+
+class Versions:
+    """A registry of writer schemas read as one reader schema: the handle deserialize_confluent_versions and
+    deserialize_single_object_versions decode with.  `writer_schemas` is a dict[int, str] by Confluent schema id
+    (rv_versions_create), or with single_object=True a list[str] keyed by the schemas' fingerprints
+    (rv_versions_create_single_object); `columns` optionally names the reader's top-level fields the batches hold."""
+
+    def __init__(self, writer_schemas, reader_schema: str, columns=None, *, single_object=False):
+        if single_object:
+            if not isinstance(writer_schemas, (list, tuple)) or not all(isinstance(sj, str) for sj in writer_schemas):
+                raise TypeError("argument 'writer_schemas': expected a list[str]")
+            self.reader = _get_or_parse_schema(reader_schema, columns)
+            full = _get_or_parse_schema(reader_schema)
+            self._writers = [_get_or_parse_schema(sj) for sj in writer_schemas]
+            n = len(self._writers)
+            hs = (ctypes.c_void_p * max(n, 1))(*[w.handle for w in self._writers])
+            names, keep = _column_names(columns) if columns is not None else (None, [])
+            h = ctypes.c_void_p()
+            _check(lib.rv_versions_create_single_object(full.handle, hs, n, names, len(keep), ctypes.byref(h)))
+            self.handle = h.value
+            return
         if not isinstance(writer_schemas, dict):
             raise TypeError("argument 'writer_schemas': expected a dict[int, str]")
         items = sorted(writer_schemas.items())
@@ -407,6 +459,34 @@ def deserialize_confluent_versions(list, writer_schemas, reader_schema, num_chun
     if not isinstance(list, type([])):
         raise TypeError("argument 'list': expected a list of bytes")
     v = _get_or_create_versions(writer_schemas, reader_schema, columns)
+    return _export_batches(_ext().decode_list_versions(v.handle, list, int(num_chunks)), v.reader)
+
+
+def deserialize_single_object_versions(list, writer_schemas, reader_schema, num_chunks=1, *, columns=None):  # noqa: A002
+    """list[bytes] of Avro single-object messages written with several schemas -> `num_chunks` RecordBatches in
+    `reader_schema`'s Arrow form, rows in message order.  `writer_schemas` (list[str]) holds every writer schema that may
+    occur; each message is decoded with the writer whose fingerprint its header names and resolved to the reader
+    (rv_decode_host_versions).  An unregistered fingerprint is an error, like a short message or a wrong C3 01 marker.
+    Two writers with the same canonical form cannot be told apart on the wire and are refused."""
+    if num_chunks < 0:
+        raise OverflowError("can't convert negative int to unsigned")
+    if not isinstance(list, type([])):
+        raise TypeError("argument 'list': expected a list of bytes")
+    if not isinstance(writer_schemas, (type([]), tuple)):
+        raise TypeError("argument 'writer_schemas': expected a list[str]")
+    if not isinstance(reader_schema, str):
+        raise TypeError("argument 'reader_schema': expected str")
+    if columns is not None:
+        if isinstance(columns, (str, bytes)):
+            raise TypeError("argument 'columns': expected a list of field names, not a single string")
+        columns = tuple(columns)
+    key = ("single_object", tuple(writer_schemas), reader_schema, columns)
+    with _schema_lock:
+        v = _versions_cache.get(key)
+    if v is None:
+        v = Versions(writer_schemas, reader_schema, columns, single_object=True)
+        with _schema_lock:
+            v = _versions_cache.setdefault(key, v)
     return _export_batches(_ext().decode_list_versions(v.handle, list, int(num_chunks)), v.reader)
 
 
@@ -530,6 +610,15 @@ def serialize_confluent(data, schema, schema_id, num_chunks=1):
     messages read back with deserialize_confluent."""
     _check_batch(data, num_chunks)
     return _export_chunks(_encode(lib.rv_encode_host_confluent, data, schema, int(num_chunks), int(schema_id)))
+
+
+def serialize_single_object(data, schema, num_chunks=1):
+    """pyarrow.RecordBatch -> `num_chunks` pyarrow Binary arrays of Avro single-object messages: element i is C3 01, the
+    little-endian CRC-64-AVRO fingerprint of `schema` (Schema.fingerprint), then row i's datum
+    (rv_encode_host_single_object).  Chunking is serialize_record_batch's; the messages read back with
+    deserialize_single_object."""
+    _check_batch(data, num_chunks)
+    return _export_chunks(_encode(lib.rv_encode_host_single_object, data, schema, int(num_chunks)))
 
 
 class _EncodedFile:

@@ -254,7 +254,11 @@ __device__ __forceinline__ int64_t init_ctx(C& c, const DecodeParams& p, const T
         if (p.frame_skip && !c.err) {  // framed input: the datum starts behind the message's header
             if (c.end - c.pos < p.frame_skip) c.err = E_FRAME;
             else {
-                if (p.frame_check) {
+                if (p.frame_check == kFrameSingleObject) {
+                    unsigned long long fp = 0;
+                    for (uint32_t b = 0; b < 8; ++b) fp |= static_cast<unsigned long long>(ld_u8(c, c.pos + 2 + b)) << (8 * b);
+                    if (ld_u8(c, c.pos) != 0xC3u || ld_u8(c, c.pos + 1) != 0x01u || fp != p.frame_fp) c.err = E_FRAME;
+                } else if (p.frame_check) {
                     const uint32_t id = (ld_u8(c, c.pos + 1) << 24) | (ld_u8(c, c.pos + 2) << 16) | (ld_u8(c, c.pos + 3) << 8) | ld_u8(c, c.pos + 4);
                     if (ld_u8(c, c.pos) != 0u || (p.frame_check == 2 && id != p.frame_id)) c.err = E_FRAME;
                 }

@@ -164,11 +164,16 @@ struct DecodeParams {
     uint32_t smem_stage_cap;  // bytes of shared memory for staging a tile's Utf8 output bytes
     int32_t count_only;       // 1: validate + totals only (no buffers yet)
     // framed input: every message starts with `frame_skip` header bytes that are not part of the datum (Confluent wire
-    // format: magic 0x00 + big-endian u32 schema id).  frame_check: 0 skip only, 1 check the magic byte, 2 also the id
+    // format: magic 0x00 + big-endian u32 schema id).  frame_check: 0 skip only, 1 check the magic byte, 2 also the id,
+    // kFrameSingleObject: Avro single-object encoding (C3 01, then the writer's CRC-64-AVRO fingerprint `frame_fp`
+    // little-endian; frame_skip = kSingleObjectHeader)
     uint32_t frame_skip;
     int32_t frame_check;
     uint32_t frame_id;
+    unsigned long long frame_fp;
 };
+constexpr int32_t kFrameSingleObject = 3;
+constexpr uint32_t kSingleObjectHeader = 10;
 
 // Object container files: where every record of every block starts (ocf.hpp, ocf_walk.cuh).
 struct OcfBlockDev { long long data_off, size, count, rec_base; };

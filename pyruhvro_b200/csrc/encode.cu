@@ -84,8 +84,8 @@ enum EncErr : uint32_t { EE_ENUM = RV_ERR_ENUM, EE_BRANCH = RV_ERR_BRANCH, EE_OV
 
 // What the write pass produces: bare datums + Binary offsets, Confluent-framed datums + Binary offsets, or the datums of
 // container blocks (no offsets: the framing kernel delimits the blocks).
-enum EncOut : int { EO_BINARY = 0, EO_CONFLUENT = 1, EO_OCF = 2 };
-constexpr uint32_t kConfluentHeader = 5;
+enum EncOut : int { EO_BINARY = 0, EO_CONFLUENT = 1, EO_OCF = 2, EO_SINGLE_OBJECT = 3 };
+constexpr uint32_t kConfluentHeader = 5;   // (single-object: kSingleObjectHeader, dev_types.h)
 
 struct EncCtx {
     const ENode* nodes;
@@ -247,7 +247,7 @@ __device__ __forceinline__ void enc_init(EncCtx& c, const EncParams& p) {
     c.pm = 1u; c.usel = 0; c.err = 0; c.size = 0; c.out = nullptr;
 }
 
-// PREFIX: bytes written in front of every datum (0, or kConfluentHeader); they count towards the row, tile and chunk sizes.
+// PREFIX: bytes written in front of every datum (0, kConfluentHeader or kSingleObjectHeader); they count towards the row, tile and chunk sizes.
 template <uint32_t PREFIX>
 __global__ void __launch_bounds__(kBlock) encode_size_kernel(const EncParams p) {
     int chunk, nrec, local; int64_t r0;
@@ -274,8 +274,10 @@ __global__ void __launch_bounds__(kBlock) encode_size_kernel(const EncParams p) 
     }
 }
 
+// fingerprint: the single-object prefix's CRC-64-AVRO (EO_SINGLE_OBJECT only).  It is a parameter of its own, not a field
+// of EncParams: the other kernels keep their parameter block, and with it their code.
 template <int OUT>
-__global__ void __launch_bounds__(kBlock) encode_write_kernel(const EncParams p) {
+__global__ void __launch_bounds__(kBlock) encode_write_kernel(const EncParams p, const unsigned long long fingerprint) {
     int chunk, nrec, local; int64_t r0;
     enc_tile(p, blockIdx.x, &chunk, &r0, &nrec, &local);
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -311,6 +313,11 @@ __global__ void __launch_bounds__(kBlock) encode_write_kernel(const EncParams p)
             c.out[1] = uint8_t(p.schema_id >> 24); c.out[2] = uint8_t(p.schema_id >> 16);
             c.out[3] = uint8_t(p.schema_id >> 8); c.out[4] = uint8_t(p.schema_id);
             c.out += kConfluentHeader;
+        }
+        if (OUT == EO_SINGLE_OBJECT) {  // C3 01, then the schema's fingerprint little-endian
+            c.out[0] = 0xC3; c.out[1] = 0x01;
+            for (int b = 0; b < 8; ++b) c.out[2 + b] = uint8_t(fingerprint >> (8 * b));
+            c.out += kSingleObjectHeader;
         }
         enc_range<1, 0>(c, 0, p.n_nodes, p.row_base + r0 + tid);
     }
@@ -675,7 +682,7 @@ struct EncGroup {
     const ArrowSchema* batch_schema;
     int64_t g0, g1, chunk_rows;
     int c0, c1, out;  // out: EncOut
-    uint32_t schema_id;
+    uint64_t key;     // EO_CONFLUENT: the schema id; EO_SINGLE_OBJECT: the fingerprint
     cudaStream_t stream;
     float* ms5;
     std::string* msg;
@@ -699,9 +706,9 @@ struct EncGroup {
     std::vector<int32_t*> h_offs;
 
     EncGroup(const AvroNode* top_, const ArrowArray* batch_, const ArrowSchema* bs, int64_t g0_, int64_t g1_, int c0_, int c1_,
-             int64_t chunk_rows_, int out_, uint32_t schema_id_, cudaStream_t stream_, float* ms5_, std::string* msg_)
+             int64_t chunk_rows_, int out_, uint64_t key_, cudaStream_t stream_, float* ms5_, std::string* msg_)
         : top(top_), batch(batch_), batch_schema(bs), g0(g0_), g1(g1_), chunk_rows(chunk_rows_), c0(c0_), c1(c1_), out(out_),
-          schema_id(schema_id_), stream(stream_), ms5(ms5_), msg(msg_) {}
+          key(key_), stream(stream_), ms5(ms5_), msg(msg_) {}
 
 #define GRP_CUDA(expr)                                                                                   \
     do {                                                                                                 \
@@ -773,7 +780,8 @@ struct EncGroup {
 
         p.nodes = static_cast<const ENode*>(d_nodes.p); p.n_nodes = int32_t(b.nodes.size());
         p.sym_off = static_cast<const int32_t*>(d_symoff.p); p.sym_bytes = static_cast<const uint8_t*>(d_symbytes.p);
-        p.n = n; p.row_base = g0; p.chunk_rows = chunk_rows; p.k = k; p.schema_id = schema_id;
+        p.n = n; p.row_base = g0; p.chunk_rows = chunk_rows; p.k = k;
+        p.schema_id = uint32_t(key);
         const int64_t tpc = std::max<int64_t>(1, (chunk_rows + kBlock - 1) / kBlock);
         const int64_t last_rows = n - chunk_rows * (k - 1);
         n_tiles = n > 0 ? tpc * (k - 1) + (last_rows + kBlock - 1) / kBlock : 0;
@@ -789,6 +797,7 @@ struct EncGroup {
             p.row_size = static_cast<uint32_t*>(d_rowsize.p); p.tile_agg = static_cast<uint32_t*>(d_agg.p);
             p.tile_base = static_cast<uint32_t*>(d_base.p); p.err = static_cast<unsigned long long*>(d_err.p);
             if (out == EO_CONFLUENT) encode_size_kernel<kConfluentHeader><<<unsigned(n_tiles), kBlock, 0, stream>>>(p);
+            else if (out == EO_SINGLE_OBJECT) encode_size_kernel<kSingleObjectHeader><<<unsigned(n_tiles), kBlock, 0, stream>>>(p);
             else encode_size_kernel<0><<<unsigned(n_tiles), kBlock, 0, stream>>>(p);
             ev.rec(2, stream);
             int thr = 32;
@@ -846,7 +855,7 @@ struct EncGroup {
         }
         p.stage_cap = uint32_t(stage);
         ev.rec(4, stream);
-        encode_write_kernel<OUT><<<unsigned(n_tiles), kBlock, stage, stream>>>(p);
+        encode_write_kernel<OUT><<<unsigned(n_tiles), kBlock, stage, stream>>>(p, key);
         return RV_OK;
     }
 
@@ -877,7 +886,8 @@ struct EncGroup {
             GRP_CUDA(cudaMemcpyAsync(static_cast<uint8_t*>(d_ptrs.p) + size_t(k) * 8, h_offs.data(), size_t(k) * 8, cudaMemcpyHostToDevice, stream));
             p.out_data = static_cast<uint8_t* const*>(d_ptrs.p);
             p.out_offsets = reinterpret_cast<int32_t* const*>(static_cast<uint8_t*>(d_ptrs.p) + size_t(k) * 8);
-            const rv_status st = out == EO_CONFLUENT ? launch_write<EO_CONFLUENT>() : launch_write<EO_BINARY>();
+            const rv_status st = out == EO_CONFLUENT ? launch_write<EO_CONFLUENT>()
+                                 : out == EO_SINGLE_OBJECT ? launch_write<EO_SINGLE_OBJECT>() : launch_write<EO_BINARY>();
             if (st) return st;
             ev.rec(5, stream);
             GRP_CUDA(cudaGetLastError());
@@ -964,10 +974,11 @@ static void for_each_group(int groups, const std::function<void(int)>& fn) {
     for (auto& t : pool) t.join();
 }
 
-// The encode behind rv_encode_host, rv_encode_host_confluent (out = EO_CONFLUENT) and rv_encode_ocf_host (ocf != null: the
+// The encode behind rv_encode_host, rv_encode_host_confluent (out = EO_CONFLUENT, key = the schema id),
+// rv_encode_host_single_object (out = EO_SINGLE_OBJECT, key = the fingerprint) and rv_encode_ocf_host (ocf != null: the
 // chunks are the file's blocks).
 static rv_status encode_batch(const rv_schema* s, const ArrowArray* batch, const ArrowSchema* batch_schema, int64_t num_chunks, int out_kind,
-                              uint32_t schema_id, const OcfSpec* ocf, rv_encoded** out) {
+                              uint64_t key, const OcfSpec* ocf, rv_encoded** out) {
     if (rv_schema_is_projection(s)) {
         rv_set_last_error("fast_encode: a column projection (rv_schema_project) or a resolved handle (rv_schema_resolve) is not a schema to write with; encode with the full schema handle");
         return RV_ERR_INVALID;
@@ -1028,7 +1039,7 @@ static rv_status encode_batch(const rv_schema* s, const ArrowArray* batch, const
         if (groups > 1 && cudaStreamCreateWithFlags(&streams[size_t(g)], cudaStreamNonBlocking) != cudaSuccess) {
             status[size_t(g)] = RV_ERR_CUDA; message[size_t(g)] = "stream creation failed"; streams[size_t(g)] = nullptr;
         }
-        grp[size_t(g)] = std::make_unique<EncGroup>(top, batch, batch_schema, g0, g1, c0, c1, chunk_rows, out_kind, schema_id, streams[size_t(g)],
+        grp[size_t(g)] = std::make_unique<EncGroup>(top, batch, batch_schema, g0, g1, c0, c1, chunk_rows, out_kind, key, streams[size_t(g)],
                                                     times[size_t(g)].data(), &message[size_t(g)]);
     }
     // one phase of group g on the group's host thread; bad_alloc there must not terminate the process
@@ -1106,6 +1117,19 @@ rv_status rv_encode_host_confluent(const rv_schema* s, struct ArrowArray* batch,
         return RV_ERR_INVALID;
     }
     return encode_batch(s, batch, batch_schema, num_chunks, EO_CONFLUENT, uint32_t(schema_id), nullptr, out);
+}
+
+rv_status rv_encode_host_single_object(const rv_schema* s, struct ArrowArray* batch, struct ArrowSchema* batch_schema, int64_t num_chunks,
+                                       rv_encoded** out) {
+    if (!s || !batch || !batch_schema || !out) { rv_set_last_error("null argument"); return RV_ERR_INVALID; }
+    *out = nullptr;
+    Releaser releaser{batch, batch_schema};
+    uint64_t fp = 0;
+    if (!rv_schema_is_projection(s)) {  // (encode_batch refuses a projected or resolved handle with its own message)
+        const rv_status st = rv_schema_fingerprint(s, &fp);
+        if (st) return st;
+    }
+    return encode_batch(s, batch, batch_schema, num_chunks, EO_SINGLE_OBJECT, fp, nullptr, out);
 }
 
 rv_status rv_encode_ocf_host(const rv_schema* s, struct ArrowArray* batch, struct ArrowSchema* batch_schema, int64_t block_records,

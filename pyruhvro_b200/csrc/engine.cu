@@ -415,6 +415,10 @@ struct rv_schema {
     // schema resolution (rv_schema_resolve): `avro` is the writer's schema, `reader` the reader's, `res` pairs them
     std::shared_ptr<const AvroNode> reader;
     std::shared_ptr<const Resolution> res;
+    // the Parsing Canonical Form of `avro` (the writer's full schema, whatever the handle's columns or reader) and its
+    // CRC-64-AVRO; canonical_why: why there is none
+    std::string canonical, canonical_why;
+    uint64_t fingerprint = 0;
     Plan plan;
     bool has_plan = false;
     std::mutex mu;
@@ -656,7 +660,26 @@ struct InputHints {
     int64_t total_bytes = -1;
     const int64_t* offsets = nullptr;  // the call's n + 1 offsets in host memory
     rv_framing framing = {0, 0, -1};   // framed input (rv_decode_*_framed)
+    bool single_object = false;        // Avro single-object input (rv_decode_*_single_object): `framing` is unused
+    uint64_t fingerprint = 0;          // ... whose header must name this writer fingerprint
 };
+
+// The record setup's check of single-object input against the writer fingerprint of `s`.
+InputHints single_object_hints(const rv_schema* s) {
+    InputHints h;
+    h.single_object = true;
+    h.fingerprint = s->fingerprint;
+    return h;
+}
+
+// RV_ERR_SCHEMA for a schema without a Parsing Canonical Form (a construct the parser keeps as unsupported).
+rv_status single_object_ok(const rv_schema* s) {
+    if (!s->canonical_why.empty()) return fail(RV_ERR_SCHEMA, "the schema has no Parsing Canonical Form: " + s->canonical_why);
+    return RV_OK;
+}
+
+constexpr const char* kSingleObjectFrameText =
+    "single-object message: shorter than its 10-byte header, not C3 01, or written with another schema (fingerprint)";
 
 // The largest input span of a tile of `tile` rows (tiles count from each chunk's first row, as tile_of does).
 int64_t max_tile_span(const int64_t* offsets, int64_t n, int64_t k, int tile) {
@@ -734,9 +757,15 @@ rv_status decode_on_device(rv_schema* s, const uint8_t* d_data, const int64_t* d
     p.sym_off = dp.sym_off; p.sym_bytes = dp.sym_bytes; p.stream_slot = dp.stream_slot;
     p.n_utf8 = 0;
     for (int i = 0; i < S; ++i) p.n_utf8 += plan.streams[size_t(i)].is_rows ? 0 : 1;
-    p.frame_skip = uint32_t(std::max(hints.framing.header_bytes, 0));
-    p.frame_check = hints.framing.check_magic ? (hints.framing.schema_id >= 0 ? 2 : 1) : 0;
-    p.frame_id = uint32_t(hints.framing.schema_id >= 0 ? hints.framing.schema_id : 0);
+    if (hints.single_object) {
+        p.frame_skip = kSingleObjectHeader;
+        p.frame_check = kFrameSingleObject;
+        p.frame_fp = hints.fingerprint;
+    } else {
+        p.frame_skip = uint32_t(std::max(hints.framing.header_bytes, 0));
+        p.frame_check = hints.framing.check_magic ? (hints.framing.schema_id >= 0 ? 2 : 1) : 0;
+        p.frame_id = uint32_t(hints.framing.schema_id >= 0 ? hints.framing.schema_id : 0);
+    }
 
     // ---- the walker and its tile; shared-memory windows: [fixed tables][input window (+pad)][Utf8 staging / scan area]
     const size_t limit = 227 * 1024;
@@ -995,7 +1024,8 @@ rv_status decode_on_device(rv_schema* s, const uint8_t* d_data, const int64_t* d
         if (err_word != ~0ull) {
             const uint32_t code = uint32_t(err_word & 0xFF);
             if (err_word_out) *err_word_out = err_word;
-            return fail(status_of(code), std::string(err_text(code)) + " (record " + std::to_string(int64_t(err_word >> 8) + record_base) + ")");
+            const char* text = code == E_FRAME && hints.single_object ? kSingleObjectFrameText : err_text(code);
+            return fail(status_of(code), std::string(text) + " (record " + std::to_string(int64_t(err_word >> 8) + record_base) + ")");
         }
         std::memcpy(chunk_tot.data(), hb_ctrl + CW_CHUNK_TOT, chunk_tot.size() * 8);
         const bool over = hb_ctrl[CW_OVER] != 0ull;
@@ -1077,6 +1107,12 @@ rv_status rv_schema_parse(const char* json, size_t len, rv_schema** out) {
         auto s = std::make_unique<rv_schema>();
         s->avro = parse_avro_schema(json, len);
         s->json.assign(json, len);
+        try {
+            s->canonical = canonical_form(*s->avro);
+            s->fingerprint = crc64_avro(s->canonical);
+        } catch (const std::exception& e) {
+            s->canonical_why = e.what();
+        }
         s->supported = is_supported(*s->avro, &s->why);
         if (s->avro->k == AK::Record) {
             try {
@@ -1139,6 +1175,7 @@ rv_status rv_schema_project(const rv_schema* s, const char* const* columns, int6
         const std::vector<int> sel = select_columns(names, requested);
         auto p = std::make_unique<rv_schema>();
         p->avro = s->avro;
+        p->canonical = s->canonical; p->canonical_why = s->canonical_why; p->fingerprint = s->fingerprint;
         p->supported = true;
         p->has_fields = true;
         p->reader = s->reader;
@@ -1172,6 +1209,7 @@ rv_status rv_schema_resolve(const rv_schema* writer, const rv_schema* reader, rv
     try {
         auto p = std::make_unique<rv_schema>();
         p->avro = writer->avro;
+        p->canonical = writer->canonical; p->canonical_why = writer->canonical_why; p->fingerprint = writer->fingerprint;
         p->reader = reader->avro;
         p->res = std::make_shared<const Resolution>(resolve_schemas(*p->avro, *p->reader));
         p->supported = true;
@@ -1184,6 +1222,25 @@ rv_status rv_schema_resolve(const rv_schema* writer, const rv_schema* reader, rv
     } catch (const std::exception& e) {
         return fail(RV_ERR_SCHEMA, e.what());
     }
+}
+
+int64_t rv_schema_canonical_form(const rv_schema* s, char* buf, size_t cap) {
+    if (!s) { fail(RV_ERR_INVALID, "null argument"); return -1; }
+    if (single_object_ok(s)) return -1;
+    if (buf && cap) {
+        const size_t n = std::min(cap - 1, s->canonical.size());
+        std::memcpy(buf, s->canonical.data(), n);
+        buf[n] = '\0';
+    }
+    return int64_t(s->canonical.size());
+}
+
+rv_status rv_schema_fingerprint(const rv_schema* s, uint64_t* out) {
+    if (!s || !out) return fail(RV_ERR_INVALID, "null argument");
+    const rv_status st = single_object_ok(s);
+    if (st) return st;
+    *out = s->fingerprint;
+    return RV_OK;
 }
 
 rv_status rv_schema_export_arrow(const rv_schema* s, struct ArrowSchema* out) {
@@ -1205,6 +1262,9 @@ static rv_status framing_ok(const rv_framing* f) {
     return RV_OK;
 }
 
+static rv_status decode_device_call(const rv_schema* s, const uint8_t* d_data, const int64_t* d_offsets, int64_t n,
+                                    int64_t num_chunks, const InputHints& hints, void* cuda_stream, rv_result** out);
+
 rv_status rv_decode_device_framed(const rv_schema* s, const uint8_t* d_data, const int64_t* d_offsets, int64_t n,
                                   int64_t num_chunks, const rv_framing* framing, void* cuda_stream, rv_result** out) {
     if (!out) return fail(RV_ERR_INVALID, "null argument");
@@ -1213,14 +1273,30 @@ rv_status rv_decode_device_framed(const rv_schema* s, const uint8_t* d_data, con
     if (st) return st;
     st = framing_ok(framing);
     if (st) return st;
+    InputHints hints;
+    if (framing) hints.framing = *framing;
+    return decode_device_call(s, d_data, d_offsets, n, num_chunks, hints, cuda_stream, out);
+}
+
+rv_status rv_decode_device_single_object(const rv_schema* s, const uint8_t* d_data, const int64_t* d_offsets, int64_t n,
+                                         int64_t num_chunks, void* cuda_stream, rv_result** out) {
+    if (!out) return fail(RV_ERR_INVALID, "null argument");
+    *out = nullptr;
+    rv_status st = check_decodable(s);
+    if (st) return st;
+    st = single_object_ok(s);
+    if (st) return st;
+    return decode_device_call(s, d_data, d_offsets, n, num_chunks, single_object_hints(s), cuda_stream, out);
+}
+
+static rv_status decode_device_call(const rv_schema* s, const uint8_t* d_data, const int64_t* d_offsets, int64_t n,
+                                    int64_t num_chunks, const InputHints& hints, void* cuda_stream, rv_result** out) {
     if (n < 0 || (n > 0 && (!d_data || !d_offsets))) return fail(RV_ERR_INVALID, "bad input pointers");
     if (reinterpret_cast<uintptr_t>(d_data) & 15u) return fail(RV_ERR_INVALID, "d_data must be 16-byte aligned");
     int device = 0;
-    st = ensure_cuda(&device);
+    rv_status st = ensure_cuda(&device);
     if (st) return st;
     cudaStream_t stream = static_cast<cudaStream_t>(cuda_stream);
-    InputHints hints;
-    if (framing) hints.framing = *framing;
     try {
         st = decode_on_device(const_cast<rv_schema*>(s), d_data, d_offsets, n, num_chunks, hints, stream, device, out);
     } catch (const std::exception& e) {
@@ -1312,11 +1388,10 @@ rv_status arena_to_host(rv_result& r, Arena& a, cudaStream_t stream, float* ms) 
 
 // H2D of rows [r0, r1) of the caller's packed input, decode into `num_chunks` batches, D2H.
 rv_status decode_host_range(rv_schema* s, const uint8_t* data, const int64_t* offsets, int64_t r0, int64_t r1, int64_t num_chunks,
-                            cudaStream_t stream, int device, rv_result** out, float* h2d_ms, float* d2h_ms, const rv_framing& framing) {
+                            cudaStream_t stream, int device, rv_result** out, float* h2d_ms, float* d2h_ms, const InputHints& frame) {
     const int64_t n = r1 - r0;
     DevBuf d_data, d_off;
-    InputHints hints;
-    hints.framing = framing;
+    InputHints hints = frame;  // (the framing of the input; the rest is this range's)
     const uint8_t* base = nullptr;
     rv_status st = RV_OK;
     if (n > 0) {
@@ -1694,6 +1769,9 @@ rv_status rv_decode_host(const rv_schema* s_, const uint8_t* data, const int64_t
     return rv_decode_host_framed(s_, data, offsets, n, num_chunks, nullptr, out);
 }
 
+static rv_status decode_host_call(rv_schema* s, const uint8_t* data, const int64_t* offsets, int64_t n, int64_t num_chunks,
+                                  const InputHints& framing, rv_result** out);
+
 rv_status rv_decode_host_framed(const rv_schema* s_, const uint8_t* data, const int64_t* offsets, int64_t n,
                                 int64_t num_chunks, const rv_framing* framing_, rv_result** out) {
     if (!out) return fail(RV_ERR_INVALID, "null argument");
@@ -1703,10 +1781,28 @@ rv_status rv_decode_host_framed(const rv_schema* s_, const uint8_t* data, const 
     if (st) return st;
     st = framing_ok(framing_);
     if (st) return st;
-    const rv_framing framing = framing_ ? *framing_ : rv_framing{0, 0, -1};
+    InputHints framing;
+    if (framing_) framing.framing = *framing_;
+    return decode_host_call(s, data, offsets, n, num_chunks, framing, out);
+}
+
+rv_status rv_decode_host_single_object(const rv_schema* s_, const uint8_t* data, const int64_t* offsets, int64_t n,
+                                       int64_t num_chunks, rv_result** out) {
+    if (!out) return fail(RV_ERR_INVALID, "null argument");
+    *out = nullptr;
+    rv_schema* s = const_cast<rv_schema*>(s_);
+    rv_status st = check_decodable(s);
+    if (st) return st;
+    st = single_object_ok(s);
+    if (st) return st;
+    return decode_host_call(s, data, offsets, n, num_chunks, single_object_hints(s), out);
+}
+
+static rv_status decode_host_call(rv_schema* s, const uint8_t* data, const int64_t* offsets, int64_t n, int64_t num_chunks,
+                                  const InputHints& framing, rv_result** out) {
     if (n < 0 || (n > 0 && (!data || !offsets))) return fail(RV_ERR_INVALID, "bad input pointers");
     int device = 0;
-    st = ensure_cuda(&device);
+    rv_status st = ensure_cuda(&device);
     if (st) return st;
     const int64_t k = clamp_chunks(num_chunks, n);
     float h2d = 0, d2h = 0;
@@ -1960,8 +2056,10 @@ const char* rv_version(void) { return "pyruhvro_b200 0.2.0 (sm_90a)"; }
 // ---- several writer schemas in one call (versions.hpp, versions.cu, DESIGN.md §7) -------------------------------------
 struct rv_versions {
     rv_schema* reader = nullptr;          // the batches' schema: the reader's, projected to the columns
-    std::vector<int64_t> ids;             // ascending
-    std::vector<rv_schema*> writers;      // the resolved (and projected) handle of ids[i]
+    bool single_object = false;           // the keys: Confluent schema ids, or single-object fingerprints
+    std::vector<int64_t> ids;             // Confluent: ascending
+    std::vector<uint64_t> fps;            // single-object: the writers' CRC-64-AVRO fingerprints, ascending
+    std::vector<rv_schema*> writers;      // the resolved (and projected) handle of ids[i] / fps[i]
     std::vector<VersionPairing> pairs;    // writers[i]'s plan next to the reader's
     ~rv_versions() {
         rv_schema_release(reader);
@@ -1972,6 +2070,20 @@ struct rv_versions {
 namespace {
 
 thread_local float t_vtimings[4] = {0, 0, 0, 0};
+
+std::string hex_fingerprint(uint64_t fp) {
+    char b[24];
+    std::snprintf(b, sizeof b, "0x%016llx", static_cast<unsigned long long>(fp));
+    return b;
+}
+
+// The framing of writer w's messages: its Confluent header, or its single-object header.
+InputHints writer_framing(const rv_versions* v, int w) {
+    if (v->single_object) return single_object_hints(v->writers[size_t(w)]);
+    InputHints h;
+    h.framing = rv_framing{5, 1, v->ids[size_t(w)]};
+    return h;
+}
 thread_local EventPool t_vevents;
 
 struct SubResults {  // the groups' one-chunk batches; their arenas go back to the cache with them
@@ -1995,7 +2107,7 @@ rv_status decode_versions(const rv_versions* v, const uint8_t* d_data, const int
                           int64_t total_bytes, cudaStream_t stream, int device, rv_result** out) {
     for (float& t : t_vtimings) t = 0;
     if (n == 0) return decode_on_device(v->reader, nullptr, nullptr, 0, num_chunks, InputHints{}, stream, device, out);
-    const int W = int(v->ids.size());
+    const int W = int(v->writers.size());
     const int64_t k64 = clamp_chunks(num_chunks, n);
     if (k64 > (int64_t(1) << 24)) return fail(RV_ERR_INVALID, "num_chunks above 2^24 is not supported");
     const int k = int(k64);
@@ -2010,7 +2122,7 @@ rv_status decode_versions(const rv_versions* v, const uint8_t* d_data, const int
     // ---- partition: count + scan, one read-back of the group sizes and the framing errors
     size_t off = 0;
     auto take_off = [&](size_t bytes) { const size_t o = off; off = align_up(off + bytes, 16); return o; };
-    const size_t o_ids = take_off(size_t(W) * 4), o_err = take_off(8 + G * 16), o_tot = o_err + 8, o_cnt = take_off(size_t(n_tiles) * W * 4),
+    const size_t o_ids = take_off(size_t(W) * 8), o_err = take_off(8 + G * 16), o_tot = o_err + 8, o_cnt = take_off(size_t(n_tiles) * W * 4),
                  o_bytes = take_off(size_t(n_tiles) * W * 8), o_msgw = take_off(size_t(n) * 2), o_map0 = take_off(size_t(n) * 8),
                  o_gdata = take_off(G * 8), o_goff = take_off(G * 8);
     DevBuf d_part, d_gdata, d_goffs, d_take;
@@ -2018,10 +2130,13 @@ rv_status decode_versions(const rv_versions* v, const uint8_t* d_data, const int
     SyncOnExit guard{stream};  // declared after the cached device blocks: runs before they go back to the cache
     uint8_t* dp = static_cast<uint8_t*>(d_part.p);
     std::vector<uint32_t> ids32(v->ids.begin(), v->ids.end());
+    const void* keys = v->single_object ? static_cast<const void*>(v->fps.data()) : ids32.data();
+    const size_t key_bytes = v->single_object ? v->fps.size() * 8 : ids32.size() * 4;
     VersionsParams p{};
     p.data = d_data; p.offsets = d_offsets; p.n = n; p.chunk_rows = chunk_rows;
     p.k = k; p.tiles_per_chunk = int32_t(tpc); p.n_tiles = int32_t(n_tiles); p.n_ids = W;
     p.ids = reinterpret_cast<const uint32_t*>(dp + o_ids);
+    p.fps = reinterpret_cast<const unsigned long long*>(dp + o_ids);
     p.err = reinterpret_cast<unsigned long long*>(dp + o_err);
     p.group_tot = reinterpret_cast<unsigned long long*>(dp + o_tot);
     p.tile_cnt = reinterpret_cast<uint32_t*>(dp + o_cnt);
@@ -2031,9 +2146,9 @@ rv_status decode_versions(const rv_versions* v, const uint8_t* d_data, const int
     p.gdata_off = reinterpret_cast<const unsigned long long*>(dp + o_gdata);
     p.goff_base = reinterpret_cast<const unsigned long long*>(dp + o_goff);
     RV_CUDA(cudaEventRecord(ev[0], stream));
-    RV_CUDA(cudaMemcpyAsync(dp + o_ids, ids32.data(), ids32.size() * 4, cudaMemcpyHostToDevice, stream));
+    RV_CUDA(cudaMemcpyAsync(dp + o_ids, keys, key_bytes, cudaMemcpyHostToDevice, stream));
     RV_CUDA(cudaMemsetAsync(dp + o_err, 0xFF, 8, stream));
-    launch_versions_partition(p, stream);
+    launch_versions_partition(p, v->single_object, stream);
     RV_CUDA(cudaGetLastError());
     std::vector<unsigned long long> back(1 + G * 2);
     RV_CUDA(cudaMemcpyAsync(back.data(), dp + o_err, back.size() * 8, cudaMemcpyDeviceToHost, stream));  // the err word, then the totals at o_tot
@@ -2049,8 +2164,7 @@ rv_status decode_versions(const rv_versions* v, const uint8_t* d_data, const int
             for (int j = 0; j < k; ++j) c += cnt(size_t(j) * W + w);
             if (c != n) continue;
             RV_CUDA(cudaEventRecord(ev[1], stream));
-            InputHints h;
-            h.framing = rv_framing{5, 1, v->ids[size_t(w)]};
+            InputHints h = writer_framing(v, w);
             h.total_bytes = total_bytes;
             const rv_status st = decode_on_device(v->writers[size_t(w)], d_data, d_offsets, n, num_chunks, h, stream, device, out);
             if (st) return st;
@@ -2090,8 +2204,7 @@ rv_status decode_versions(const rv_versions* v, const uint8_t* d_data, const int
     for (size_t g = 0; g < G; ++g) {
         if (cnt(g) == 0) continue;
         const int j = int(g / size_t(W)), w = int(g % size_t(W));
-        InputHints h;
-        h.framing = rv_framing{5, 1, v->ids[size_t(w)]};
+        InputHints h = writer_framing(v, w);
         h.total_bytes = bytes(g);
         unsigned long long ew = ~0ull;
         const rv_status st = decode_on_device(v->writers[size_t(w)], p.gdata + gdata_off[g], p.goffs + goff_base[g], cnt(g), 1, h, stream,
@@ -2108,15 +2221,22 @@ rv_status decode_versions(const rv_versions* v, const uint8_t* d_data, const int
         const int64_t rec = int64_t(best >> 8);
         if (code == E_FRAME_ID) {
             int64_t a = 0;
-            uint8_t hdr[5] = {0, 0, 0, 0, 0};
+            uint8_t hdr[kSingleObjectHeader] = {};
             RV_CUDA(cudaMemcpyAsync(&a, d_offsets + rec, 8, cudaMemcpyDeviceToHost, stream));
             RV_CUDA(cudaStreamSynchronize(stream));
-            RV_CUDA(cudaMemcpyAsync(hdr, d_data + a, 5, cudaMemcpyDeviceToHost, stream));
+            RV_CUDA(cudaMemcpyAsync(hdr, d_data + a, v->single_object ? kSingleObjectHeader : 5, cudaMemcpyDeviceToHost, stream));
             RV_CUDA(cudaStreamSynchronize(stream));
+            if (v->single_object) {
+                uint64_t fp = 0;
+                for (int b = 0; b < 8; ++b) fp |= uint64_t(hdr[2 + b]) << (8 * b);
+                return fail(RV_ERR_FRAME, "single-object message: schema fingerprint " + hex_fingerprint(fp) + " is not registered (record " +
+                                              std::to_string(rec) + ")");
+            }
             const uint32_t id = (uint32_t(hdr[1]) << 24) | (uint32_t(hdr[2]) << 16) | (uint32_t(hdr[3]) << 8) | uint32_t(hdr[4]);
             return fail(RV_ERR_FRAME, "framed message: schema id " + std::to_string(id) + " is not registered (record " + std::to_string(rec) + ")");
         }
-        return fail(status_of(code), std::string(err_text(code)) + " (record " + std::to_string(rec) + ")");
+        const char* text = code == E_FRAME && v->single_object ? kSingleObjectFrameText : err_text(code);
+        return fail(status_of(code), std::string(text) + " (record " + std::to_string(rec) + ")");
     }
 
     // ---- the output batches' exact layout: sums over each chunk's groups
@@ -2180,6 +2300,41 @@ rv_status check_versions_input(const rv_versions* v, int64_t n, bool have_ptrs, 
     return RV_OK;
 }
 
+// The writers of `v` (its keys already in place, in `order`) resolved to the reader and projected to `columns`.
+rv_status register_writers(const rv_schema* reader, const rv_schema* const* writers, const std::vector<size_t>& order,
+                           const char* const* columns, int64_t n_columns, std::unique_ptr<rv_versions> v, rv_versions** out) {
+    rv_status st = check_decodable(reader);
+    if (st) return st;
+    if (columns) {
+        st = rv_schema_project(reader, columns, n_columns, &v->reader);
+        if (st) return st;
+    } else {
+        v->reader = rv_schema_retain(const_cast<rv_schema*>(reader));
+    }
+    for (size_t q = 0; q < order.size(); ++q) {
+        const size_t i = order[q];
+        const std::string who = v->single_object ? "writer " + std::to_string(i) + " (fingerprint " + hex_fingerprint(v->fps[q]) + "): "
+                                                 : "schema id " + std::to_string(v->ids[q]) + ": ";
+        rv_schema* r = nullptr;
+        st = rv_schema_resolve(writers[i], reader, &r);
+        if (st) return fail(st, who + t_error);
+        if (columns) {
+            rv_schema* full = r;
+            st = rv_schema_project(full, columns, n_columns, &r);
+            rv_schema_release(full);
+            if (st) return fail(st, who + t_error);
+        }
+        v->writers.push_back(r);
+        try {
+            v->pairs.push_back(pair_plans(v->reader->plan, r->plan));
+        } catch (const std::exception& e) {
+            return fail(RV_ERR_SCHEMA, who + e.what());
+        }
+    }
+    *out = v.release();
+    return RV_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -2207,37 +2362,40 @@ rv_status rv_versions_create(const rv_schema* reader, const int64_t* schema_ids,
     for (size_t i = 1; i < order.size(); ++i)
         if (schema_ids[order[i]] == schema_ids[order[i - 1]])
             return fail(RV_ERR_INVALID, "schema versions: schema id " + std::to_string(schema_ids[order[i]]) + " is registered twice");
-    rv_status st = check_decodable(reader);
-    if (st) return st;
     auto v = std::make_unique<rv_versions>();
-    if (columns) {
-        st = rv_schema_project(reader, columns, n_columns, &v->reader);
-        if (st) return st;
-    } else {
-        v->reader = rv_schema_retain(const_cast<rv_schema*>(reader));
-    }
-    for (size_t i : order) {
-        const std::string who = "schema id " + std::to_string(schema_ids[i]) + ": ";
-        rv_schema* r = nullptr;
-        st = rv_schema_resolve(writers[i], reader, &r);
-        if (st) return fail(st, who + t_error);
-        if (columns) {
-            rv_schema* full = r;
-            st = rv_schema_project(full, columns, n_columns, &r);
-            rv_schema_release(full);
-            if (st) return fail(st, who + t_error);
-        }
-        v->ids.push_back(schema_ids[i]);
-        v->writers.push_back(r);
-        try {
-            v->pairs.push_back(pair_plans(v->reader->plan, r->plan));
-        } catch (const std::exception& e) {
-            return fail(RV_ERR_SCHEMA, who + e.what());
-        }
-    }
-    *out = v.release();
-    return RV_OK;
+    for (size_t i : order) v->ids.push_back(schema_ids[i]);
+    return register_writers(reader, writers, order, columns, n_columns, std::move(v), out);
 }
+
+rv_status rv_versions_create_single_object(const rv_schema* reader, const rv_schema* const* writers, int64_t n_writers,
+                                           const char* const* columns, int64_t n_columns, rv_versions** out) {
+    if (!out) return fail(RV_ERR_INVALID, "null argument");
+    *out = nullptr;
+    if (!reader || (n_writers > 0 && !writers) || (!columns && n_columns != 0) || n_columns < 0) return fail(RV_ERR_INVALID, "null argument");
+    if (n_writers < 1) return fail(RV_ERR_INVALID, "schema versions: no writer schemas");
+    if (n_writers > kMaxVersions) return fail(RV_ERR_INVALID, "schema versions: more than " + std::to_string(kMaxVersions) + " writer schemas");
+    auto bad_handle = [](const rv_schema* s) { return !s || !s->keep.empty() || s->res; };
+    if (bad_handle(reader)) return fail(RV_ERR_INVALID, "schema versions: pass the handle of the reader's full schema (rv_schema_parse)");
+    std::vector<size_t> order(static_cast<size_t>(n_writers));
+    for (int64_t i = 0; i < n_writers; ++i) {
+        order[size_t(i)] = size_t(i);
+        if (bad_handle(writers[i]))
+            return fail(RV_ERR_INVALID, "schema versions: pass the handles of the writers' full schemas (rv_schema_parse), writer " + std::to_string(i));
+        if (!writers[i]->canonical_why.empty())
+            return fail(RV_ERR_SCHEMA, "schema versions: writer " + std::to_string(i) + " has no Parsing Canonical Form: " + writers[i]->canonical_why);
+    }
+    std::sort(order.begin(), order.end(), [&](size_t a, size_t b) { return writers[a]->fingerprint < writers[b]->fingerprint; });
+    for (size_t i = 1; i < order.size(); ++i)
+        if (writers[order[i]]->fingerprint == writers[order[i - 1]]->fingerprint)
+            return fail(RV_ERR_INVALID, "schema versions: writers " + std::to_string(std::min(order[i], order[i - 1])) + " and " +
+                                            std::to_string(std::max(order[i], order[i - 1])) + " have the same fingerprint " +
+                                            hex_fingerprint(writers[order[i]]->fingerprint) + " (their canonical forms are equal)");
+    auto v = std::make_unique<rv_versions>();
+    v->single_object = true;
+    for (size_t i : order) v->fps.push_back(writers[i]->fingerprint);
+    return register_writers(reader, writers, order, columns, n_columns, std::move(v), out);
+}
+
 
 void rv_versions_release(rv_versions* v) { delete v; }
 

@@ -42,7 +42,7 @@ void launch_ocf_offsets(const OcfParams& q, cudaStream_t s);
 void launch_gather_push(const PushJob* jobs, int n_jobs, int parts, cudaStream_t s);
 // multi-version Confluent decode (versions.cu): count + scan of the partition, then (after the host placed the groups)
 // the scatter; one level of row spaces of the take
-void launch_versions_partition(const VersionsParams& p, cudaStream_t s);
+void launch_versions_partition(const VersionsParams& p, bool single_object, cudaStream_t s);  // keys: p.ids, or p.fps
 void launch_versions_scatter(const VersionsParams& p, cudaStream_t s);
 void launch_take_level(const TakeSpace* spaces, int n_spaces, long long blocks, const TakeJob* jobs, const TakeScan* scans, int n_scans,
                        cudaStream_t s);

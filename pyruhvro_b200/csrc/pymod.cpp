@@ -132,13 +132,10 @@ struct PinnedPair {  // the two slabs of one call
     ~PinnedPair() { rv_host_free(a); rv_host_free(b); }
 };
 
-// decode_list(schema_handle: int, records: list[bytes], num_chunks: int) -> result handle (int)
-PyObject* decode_list(PyObject*, PyObject* args) {
-    unsigned long long schema_addr = 0;
-    PyObject* list = nullptr;
-    long long num_chunks = 1, header_bytes = 0, check_magic = 0, schema_id = -1;
-    if (!PyArg_ParseTuple(args, "KO!L|LLL", &schema_addr, &PyList_Type, &list, &num_chunks, &header_bytes, &check_magic, &schema_id)) return nullptr;
-    const rv_schema* schema = reinterpret_cast<const rv_schema*>(static_cast<uintptr_t>(schema_addr));
+// The pinned gather of `list`, then decode(data, offsets, n, &result) without the GIL (py.detach, src/lib.rs:64-69,82-87).
+// Returns the result handle (int), or nullptr with the Python error set.
+template <class Decode>
+PyObject* decode_gathered(PyObject* list, Decode&& decode) {
     PinnedPair slabs;
     Packed pk;
     bool first = true;
@@ -156,10 +153,8 @@ PyObject* decode_list(PyObject*, PyObject* args) {
     }
     rv_result* result = nullptr;
     rv_status st = RV_OK;
-    Py_BEGIN_ALLOW_THREADS;  // py.detach (src/lib.rs:64-69,82-87): the decode runs without the GIL
-    const rv_framing framing = {int32_t(header_bytes), int32_t(check_magic), int64_t(schema_id)};
-    st = rv_decode_host_framed(schema, reinterpret_cast<const uint8_t*>(pk.data), pk.offsets, pk.n, num_chunks,
-                               header_bytes > 0 ? &framing : nullptr, &result);
+    Py_BEGIN_ALLOW_THREADS;
+    st = decode(reinterpret_cast<const uint8_t*>(pk.data), pk.offsets, pk.n, &result);
     Py_END_ALLOW_THREADS;
     if (st != RV_OK) {
         PyErr_SetString(PyExc_ValueError, rv_last_error());
@@ -168,39 +163,43 @@ PyObject* decode_list(PyObject*, PyObject* args) {
     return PyLong_FromUnsignedLongLong(static_cast<unsigned long long>(reinterpret_cast<uintptr_t>(result)));
 }
 
-// decode_list_versions(versions_handle: int, records: list[bytes], num_chunks: int) -> result handle (int): Confluent
-// messages of several writer schemas (rv_decode_host_versions), through the same pinned gather as decode_list
+// decode_list(schema_handle: int, records: list[bytes], num_chunks: int) -> result handle (int)
+PyObject* decode_list(PyObject*, PyObject* args) {
+    unsigned long long schema_addr = 0;
+    PyObject* list = nullptr;
+    long long num_chunks = 1, header_bytes = 0, check_magic = 0, schema_id = -1;
+    if (!PyArg_ParseTuple(args, "KO!L|LLL", &schema_addr, &PyList_Type, &list, &num_chunks, &header_bytes, &check_magic, &schema_id)) return nullptr;
+    const rv_schema* schema = reinterpret_cast<const rv_schema*>(static_cast<uintptr_t>(schema_addr));
+    const rv_framing framing = {int32_t(header_bytes), int32_t(check_magic), int64_t(schema_id)};
+    return decode_gathered(list, [&](const uint8_t* data, const int64_t* offsets, int64_t n, rv_result** out) {
+        return rv_decode_host_framed(schema, data, offsets, n, num_chunks, header_bytes > 0 ? &framing : nullptr, out);
+    });
+}
+
+// decode_list_versions(versions_handle: int, records: list[bytes], num_chunks: int) -> result handle (int): Confluent or
+// single-object messages of several writer schemas (rv_decode_host_versions), through the same pinned gather as decode_list
 PyObject* decode_list_versions(PyObject*, PyObject* args) {
     unsigned long long addr = 0;
     PyObject* list = nullptr;
     long long num_chunks = 1;
     if (!PyArg_ParseTuple(args, "KO!L", &addr, &PyList_Type, &list, &num_chunks)) return nullptr;
     const rv_versions* v = reinterpret_cast<const rv_versions*>(static_cast<uintptr_t>(addr));
-    PinnedPair slabs;
-    Packed pk;
-    bool first = true;
-    auto alloc = [&](size_t bytes) -> void* {
-        void* p = rv_host_alloc(bytes);
-        (first ? slabs.a : slabs.b) = p;
-        first = false;
-        return p;
-    };
-    try {
-        if (!pack_list(list, alloc, &pk)) return nullptr;
-    } catch (const std::exception& e) {
-        PyErr_SetString(PyExc_MemoryError, e.what());
-        return nullptr;
-    }
-    rv_result* result = nullptr;
-    rv_status st = RV_OK;
-    Py_BEGIN_ALLOW_THREADS;
-    st = rv_decode_host_versions(v, reinterpret_cast<const uint8_t*>(pk.data), pk.offsets, pk.n, num_chunks, &result);
-    Py_END_ALLOW_THREADS;
-    if (st != RV_OK) {
-        PyErr_SetString(PyExc_ValueError, rv_last_error());
-        return nullptr;
-    }
-    return PyLong_FromUnsignedLongLong(static_cast<unsigned long long>(reinterpret_cast<uintptr_t>(result)));
+    return decode_gathered(list, [&](const uint8_t* data, const int64_t* offsets, int64_t n, rv_result** out) {
+        return rv_decode_host_versions(v, data, offsets, n, num_chunks, out);
+    });
+}
+
+// decode_list_single_object(schema_handle: int, records: list[bytes], num_chunks: int) -> result handle (int): Avro
+// single-object messages of one writer schema (rv_decode_host_single_object)
+PyObject* decode_list_single_object(PyObject*, PyObject* args) {
+    unsigned long long schema_addr = 0;
+    PyObject* list = nullptr;
+    long long num_chunks = 1;
+    if (!PyArg_ParseTuple(args, "KO!L", &schema_addr, &PyList_Type, &list, &num_chunks)) return nullptr;
+    const rv_schema* schema = reinterpret_cast<const rv_schema*>(static_cast<uintptr_t>(schema_addr));
+    return decode_gathered(list, [&](const uint8_t* data, const int64_t* offsets, int64_t n, rv_result** out) {
+        return rv_decode_host_single_object(schema, data, offsets, n, num_chunks, out);
+    });
 }
 
 // pack(records: list[bytes]) -> (data: bytes, offsets: bytes of int64[n+1]).  The packing step alone, into ordinary
@@ -228,6 +227,7 @@ PyObject* pack(PyObject*, PyObject* args) {
 PyMethodDef methods[] = {
     {"decode_list", decode_list, METH_VARARGS, "decode_list(schema_handle, records: list[bytes], num_chunks[, header_bytes, check_magic, schema_id]) -> result handle"},
     {"decode_list_versions", decode_list_versions, METH_VARARGS, "decode_list_versions(versions_handle, records: list[bytes], num_chunks) -> result handle"},
+    {"decode_list_single_object", decode_list_single_object, METH_VARARGS, "decode_list_single_object(schema_handle, records: list[bytes], num_chunks) -> result handle"},
     {"pack", pack, METH_VARARGS, "pack(records: list[bytes]) -> (data, offsets): the packing step alone (test hook)"},
     {nullptr, nullptr, 0, nullptr},
 };

@@ -2,6 +2,7 @@
 #include "schema.hpp"
 
 #include <algorithm>
+#include <array>
 #include <cerrno>
 #include <climits>
 #include <cmath>
@@ -837,6 +838,87 @@ Resolution resolve_node(const AvroNode& w, const AvroNode& r, const std::string&
 Resolution resolve_schemas(const AvroNode& writer, const AvroNode& reader) {
     if (writer.k != AK::Record || reader.k != AK::Record) throw std::runtime_error("schema resolution: both schemas must be records");
     return resolve_node(writer, reader, std::string());
+}
+
+// ---- Parsing Canonical Form and CRC-64-AVRO (the specification's "Schema Fingerprints") -------------------------------
+namespace {
+
+// The parser replaces a reference by a copy of the definition it names, so a named type met again is written as its
+// fullname here, as the reference was.
+void canonical_node(const AvroNode& n, std::set<std::string>& named, std::string& o) {
+    auto named_head = [&](const char* type) -> bool {  // false: already written, the fullname alone
+        if (!named.insert(n.fullname).second) { o += "\"" + n.fullname + "\""; return false; }
+        o += "{\"name\":\"" + n.fullname + "\",\"type\":\"" + type + "\"";
+        return true;
+    };
+    switch (n.k) {
+        case AK::Null: o += "\"null\""; return;
+        case AK::Bool: o += "\"boolean\""; return;
+        case AK::Int: case AK::Date: case AK::TimeMillis: o += "\"int\""; return;
+        case AK::Long: case AK::TsMillis: case AK::TsMicros: case AK::TimeMicros: o += "\"long\""; return;
+        case AK::Float: o += "\"float\""; return;
+        case AK::Double: o += "\"double\""; return;
+        case AK::String: case AK::Uuid: o += "\"string\""; return;
+        case AK::Bytes: case AK::DecimalBytes: o += "\"bytes\""; return;
+        case AK::Fixed: case AK::DecimalFixed:
+            if (named_head("fixed")) o += ",\"size\":" + std::to_string(n.size) + "}";
+            return;
+        case AK::Enum:
+            if (!named_head("enum")) return;
+            o += ",\"symbols\":[";
+            for (size_t i = 0; i < n.symbols.size(); ++i) o += (i ? ",\"" : "\"") + n.symbols[i] + "\"";
+            o += "]}";
+            return;
+        case AK::Record:
+            if (!named_head("record")) return;
+            o += ",\"fields\":[";
+            for (size_t i = 0; i < n.fields.size(); ++i) {
+                o += (i ? ",{\"name\":\"" : "{\"name\":\"") + n.fields[i].name + "\",\"type\":";
+                canonical_node(*n.fields[i].type, named, o);
+                o += "}";
+            }
+            o += "]}";
+            return;
+        case AK::Union:
+            o += "[";
+            for (size_t i = 0; i < n.sub.size(); ++i) {
+                if (i) o += ",";
+                canonical_node(*n.sub[i], named, o);
+            }
+            o += "]";
+            return;
+        case AK::Array: case AK::Map:
+            o += n.k == AK::Array ? "{\"type\":\"array\",\"items\":" : "{\"type\":\"map\",\"values\":";
+            canonical_node(*n.sub[0], named, o);
+            o += "}";
+            return;
+        case AK::Unsupported:
+            throw std::runtime_error("Parsing Canonical Form: unsupported type: " + n.what);
+    }
+}
+
+}  // namespace
+
+std::string canonical_form(const AvroNode& top) {
+    std::set<std::string> named;
+    std::string o;
+    canonical_node(top, named, o);
+    return o;
+}
+
+uint64_t crc64_avro(const std::string& bytes) {
+    static const auto table = [] {
+        std::array<uint64_t, 256> t{};
+        for (uint64_t i = 0; i < 256; ++i) {
+            uint64_t fp = i;
+            for (int j = 0; j < 8; ++j) fp = (fp >> 1) ^ (kCrc64AvroEmpty & (0 - (fp & 1)));
+            t[size_t(i)] = fp;
+        }
+        return t;
+    }();
+    uint64_t fp = kCrc64AvroEmpty;
+    for (unsigned char b : bytes) fp = (fp >> 8) ^ table[size_t((fp ^ b) & 0xFF)];
+    return fp;
 }
 
 }  // namespace rv

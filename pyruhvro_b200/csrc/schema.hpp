@@ -106,4 +106,15 @@ struct Resolution {
 // and the host emulation both build from it.
 Resolution resolve_schemas(const AvroNode& writer, const AvroNode& reader);
 
+// ---- schema fingerprints (the specification's "Parsing Canonical Form" and "Schema Fingerprints") --------------------
+// The canonical form of a parsed schema: primitives as bare names, named types by fullname (written in full at their
+// first occurrence, by fullname after that), only name / type / fields / symbols / items / values / size in that order,
+// logical types, docs, aliases and defaults dropped, no whitespace.  Throws std::runtime_error for a schema the parser
+// keeps as AK::Unsupported (its underlying type is not kept).
+std::string canonical_form(const AvroNode& top);
+
+// CRC-64-AVRO of `bytes`: the 64-bit Rabin fingerprint the single-object encoding names its writer schema by.
+constexpr uint64_t kCrc64AvroEmpty = 0xc15d213aa4d7a795ull;
+uint64_t crc64_avro(const std::string& bytes);
+
 }  // namespace rv

@@ -18,7 +18,7 @@
 namespace rv {
 
 constexpr int kMaxVersions = 256;   // registered writer schemas of one rv_versions handle (the partition's id table)
-constexpr uint32_t E_FRAME_ID = 14; // framed message whose schema id is not registered (reported as RV_ERR_FRAME)
+constexpr uint32_t E_FRAME_ID = 14; // framed message whose schema id / fingerprint is not registered (reported as RV_ERR_FRAME)
 constexpr unsigned long long kNoRow = ~0ull;  // row-map entry of a message that failed its header check
 
 // A row-map entry: output row -> (writer index, row within that writer's part of the chunk).
@@ -37,6 +37,22 @@ RV_HD uint32_t vp_header(const uint8_t* m, int64_t len, const uint32_t* ids, int
         if (ids[mid] < id) lo = mid + 1; else hi = mid;
     }
     if (lo == n_ids || ids[lo] != id) return E_FRAME_ID;
+    *writer = lo;
+    return E_OK;
+}
+
+// The single-object header of message [m, m + len): C3 01, then the little-endian CRC-64-AVRO fingerprint of the
+// writer's schema, looked up in the sorted table fps[0 .. n_fps).  Returns like the Confluent vp_header.
+RV_HD uint32_t vp_header(const uint8_t* m, int64_t len, const unsigned long long* fps, int n_fps, int* writer) {
+    if (len < int64_t(kSingleObjectHeader) || m[0] != 0xC3u || m[1] != 0x01u) return E_FRAME;
+    unsigned long long fp = 0;
+    for (int b = 0; b < 8; ++b) fp |= static_cast<unsigned long long>(m[2 + b]) << (8 * b);
+    int lo = 0, hi = n_fps;
+    while (lo < hi) {
+        const int mid = (lo + hi) >> 1;
+        if (fps[mid] < fp) lo = mid + 1; else hi = mid;
+    }
+    if (lo == n_fps || fps[lo] != fp) return E_FRAME_ID;
     *writer = lo;
     return E_OK;
 }
@@ -96,6 +112,7 @@ struct VersionsParams {
     int64_t* goffs;                      // the groups' offsets
     const unsigned long long* goff_base; // [k][W] where group g's rows + 1 offsets start in goffs
     unsigned long long* map0;            // [n] space-0 row map (take_pack)
+    const unsigned long long* fps;       // [W] single-object registries: the writers' fingerprints, ascending (instead of ids)
 };
 
 // Validity / Bits: the source row's bit (a missing validity buffer counts as all valid).

@@ -1,7 +1,8 @@
 // sm_90a kernels of the multi-version Confluent decode (rv_decode_*_versions, DESIGN.md §7 "Several writer schemas").
 //
-//   vp_count_kernel    one lane per message: the Confluent header, the schema id's writer (binary search in the
-//                      registered ids, staged in shared memory), per tile the messages and bytes of every writer
+//   vp_count_kernel    one lane per message: the Confluent or single-object header, the writer of its schema id or
+//                      fingerprint (binary search in the registered keys, staged in shared memory), per tile the
+//                      messages and bytes of every writer
 //   vp_scan_kernel     one CTA per (output chunk, writer): the tiles' counts scanned into bases, the group's totals
 //   vp_scatter_kernel  one lane per message: its rank in its group (warp shuffles + per-warp totals in shared memory),
 //                      the group's i64 offsets, the space-0 row map; each warp copies its messages' bytes together
@@ -31,12 +32,21 @@ __device__ __forceinline__ TileRange tile_range(const VersionsParams& p, int t) 
     return tr;
 }
 
+// Key: uint32_t (Confluent schema ids, p.ids) or unsigned long long (single-object fingerprints, p.fps).
+template <class Key>
+__device__ __forceinline__ const Key* vp_keys(const VersionsParams& p);
+template <>
+__device__ __forceinline__ const uint32_t* vp_keys<uint32_t>(const VersionsParams& p) { return p.ids; }
+template <>
+__device__ __forceinline__ const unsigned long long* vp_keys<unsigned long long>(const VersionsParams& p) { return p.fps; }
+
+template <class Key>
 __global__ void __launch_bounds__(kTakeBlock) vp_count_kernel(const VersionsParams p) {
-    __shared__ uint32_t s_ids[kMaxVersions];
+    __shared__ Key s_ids[kMaxVersions];
     __shared__ uint32_t s_cnt[kMaxVersions];
     __shared__ unsigned long long s_bytes[kMaxVersions];
     const int W = p.n_ids;
-    for (int w = threadIdx.x; w < W; w += kTakeBlock) { s_ids[w] = p.ids[w]; s_cnt[w] = 0; s_bytes[w] = 0; }
+    for (int w = threadIdx.x; w < W; w += kTakeBlock) { s_ids[w] = vp_keys<Key>(p)[w]; s_cnt[w] = 0; s_bytes[w] = 0; }
     __syncthreads();
     const TileRange tr = tile_range(p, int(blockIdx.x));
     const int64_t row = tr.r0 + threadIdx.x;
@@ -238,8 +248,9 @@ __global__ void __launch_bounds__(kTakeBlock) take_offsets_kernel(const TakeSpac
 
 }  // namespace
 
-void launch_versions_partition(const VersionsParams& p, cudaStream_t s) {
-    vp_count_kernel<<<unsigned(p.n_tiles), kTakeBlock, 0, s>>>(p);
+void launch_versions_partition(const VersionsParams& p, bool single_object, cudaStream_t s) {
+    if (single_object) vp_count_kernel<unsigned long long><<<unsigned(p.n_tiles), kTakeBlock, 0, s>>>(p);
+    else vp_count_kernel<uint32_t><<<unsigned(p.n_tiles), kTakeBlock, 0, s>>>(p);
     vp_scan_kernel<<<dim3(static_cast<unsigned>(p.k), static_cast<unsigned>(p.n_ids)), kTakeBlock, 0, s>>>(p);
 }
 
