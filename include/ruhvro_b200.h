@@ -107,6 +107,22 @@ rv_status rv_schema_project(const rv_schema* s, const char* const* columns, int6
  * passed as writer or reader. */
 rv_status rv_schema_resolve(const rv_schema* writer, const rv_schema* reader, rv_schema** out);
 
+/* A permissive handle: decodes that do not fail on a damaged record.  Let R be the output schema of `s` (plain,
+ * projected or resolved) and R' be R with every top-level field whose type is not a union, null or a map made optional
+ * (T -> ["null", T]; a reader-only field with a non-null default -> [T, "null"], the same Arrow column; a nullable map
+ * has no Arrow form here).  Every
+ * rv_decode_{host,device}[_framed|_single_object] entry point takes the handle.  Each record whose strict decode alone
+ * fails with RV_ERR_EOF, _VARINT, _BOOL, _NEG_LEN, _BRANCH, _ENUM (an unmapped enum symbol included), _VALUE or _FRAME
+ * becomes a bad row: null in every top-level column (a map column: an empty map; an N-variant union column: type id 0
+ * and absent children), listed by rv_result_bad.  Other rows hold the strict decode's values; the k batches keep the strict call's row counts, so
+ * rows stay aligned with the input messages.  RV_ERR_OVERFLOW, RV_ERR_SCHEMA, RV_ERR_INVALID and RV_ERR_CUDA still
+ * fail the call.  The batches are, buffer for buffer, the plain decode with R' of the input in which every good record
+ * is re-encoded with R' and every bad one is the datum with branch null in each optional top-level field.
+ * rv_schema_export_arrow gives R'; the canonical form and fingerprint stay the writer's.  rv_schema_project of a
+ * permissive handle stays permissive.  RV_ERR_INVALID: `s` is already permissive.  rv_versions_create*, rv_encode_*
+ * and rv_encode_ocf_host refuse a permissive handle (RV_ERR_INVALID). */
+rv_status rv_schema_permissive(const rv_schema* s, rv_schema** out);
+
 /* The Avro specification's Parsing Canonical Form of the schema and its CRC-64-AVRO fingerprint (the 64-bit Rabin
  * fingerprint, EMPTY = 0xc15d213aa4d7a795), the key single-object encoding names a writer schema by.  The form keeps
  * primitives as bare names, named types by fullname (in full at their first occurrence, by fullname after that), only
@@ -246,6 +262,14 @@ int64_t rv_result_num_batches(const rv_result* r);
 int64_t rv_result_num_rows(const rv_result* r, int64_t batch);
 /* Exact bytes of every Arrow buffer that is exported (the B_out of the roofline bookkeeping). */
 int64_t rv_result_arrow_bytes(const rv_result* r);
+
+/* Permissive decodes (rv_schema_permissive): the bad records of the call, in record order.  rv_result_bad copies at most
+ * `cap` of them (record index in the call, rv_status of the record's strict decode) and returns how many there are
+ * (-1: a null argument with cap > 0).  rv_result_bad_message gives entry i's message: the strict call's message
+ * without " (record N)" (NULL: no such entry).  A strict decode has none. */
+int64_t rv_result_num_bad(const rv_result* r);
+int64_t rv_result_bad(const rv_result* r, int64_t* records, int32_t* status, int64_t cap);
+const char* rv_result_bad_message(const rv_result* r, int64_t i);
 
 /* Bytes of the result's buffer arena (what rv_result_to_host copies over PCIe; includes 64-byte
  * padding and validity bitmaps that end up not being exported). */

@@ -103,6 +103,13 @@ def _bind(L):
     L.rv_result_num_rows.argtypes = [vp, i64]
     L.rv_result_arrow_bytes.restype = i64
     L.rv_result_arrow_bytes.argtypes = [vp]
+    L.rv_schema_permissive.argtypes = [vp, ctypes.POINTER(vp)]
+    L.rv_result_num_bad.restype = i64
+    L.rv_result_num_bad.argtypes = [vp]
+    L.rv_result_bad.restype = i64
+    L.rv_result_bad.argtypes = [vp, vp, vp, i64]
+    L.rv_result_bad_message.restype = ctypes.c_char_p
+    L.rv_result_bad_message.argtypes = [vp, i64]
     L.rv_result_buffer_bytes.restype = i64
     L.rv_result_buffer_bytes.argtypes = [vp]
     L.rv_result_export.argtypes = [vp, i64, vp, vp]
@@ -204,6 +211,14 @@ class Schema:
         _check(lib.rv_schema_resolve(self.handle, reader.handle, ctypes.byref(h)))
         return Schema._adopt(h.value)
 
+    def permissive(self) -> "Schema":
+        """A schema whose decodes turn a damaged record into a null row instead of failing (rv_schema_permissive).  Its
+        batches are this schema's with every top-level field that is not a union, null or a map made nullable; the bad
+        records are reported with the batches (errors="null" of the decode functions)."""
+        h = ctypes.c_void_p()
+        _check(lib.rv_schema_permissive(self.handle, ctypes.byref(h)))
+        return Schema._adopt(h.value)
+
     @property
     def canonical_form(self) -> str:
         """The Avro specification's Parsing Canonical Form of the writer's full schema (also for a projected or resolved
@@ -267,7 +282,7 @@ _schema_cache = {}
 _schema_lock = threading.Lock()
 
 
-def _get_or_parse_schema(schema: str, columns=None, reader_schema=None) -> Schema:
+def _get_or_parse_schema(schema: str, columns=None, reader_schema=None, permissive=False) -> Schema:
     if not isinstance(schema, str):
         raise TypeError("argument 'schema': expected str")
     if reader_schema is not None and not isinstance(reader_schema, str):
@@ -276,12 +291,14 @@ def _get_or_parse_schema(schema: str, columns=None, reader_schema=None) -> Schem
         if isinstance(columns, (str, bytes)):
             raise TypeError("argument 'columns': expected a list of field names, not a single string")
         columns = tuple(columns)
-    key = (schema, reader_schema, columns)
+    key = (schema, reader_schema, columns, permissive)
     with _schema_lock:
         s = _schema_cache.get(key)
     if s is not None:
         return s
-    if columns is not None:
+    if permissive:
+        parsed = _get_or_parse_schema(schema, columns, reader_schema).permissive()
+    elif columns is not None:
         parsed = _get_or_parse_schema(schema, None, reader_schema).project(columns)
     elif reader_schema is not None:
         parsed = _get_or_parse_schema(schema).read_as(reader_schema)
@@ -291,9 +308,9 @@ def _get_or_parse_schema(schema: str, columns=None, reader_schema=None) -> Schem
         return _schema_cache.setdefault(key, parsed)
 
 
-def _export_batches(result_handle: int, schema: Schema) -> List[pa.RecordBatch]:
+def _export_batches(result_handle: int, schema: Schema, with_bad: bool = False):
     """rv_result -> pyarrow batches through the Arrow C Data Interface; frees the result handle
-    (the exported arrays keep the underlying memory alive)."""
+    (the exported arrays keep the underlying memory alive).  with_bad: (batches, the bad-record report)."""
     try:
         arrow_schema = schema.arrow_schema
         out = []
@@ -301,9 +318,34 @@ def _export_batches(result_handle: int, schema: Schema) -> List[pa.RecordBatch]:
             arr = _ArrowArray()
             _check(lib.rv_result_export(result_handle, i, ctypes.addressof(arr), None))
             out.append(pa.RecordBatch._import_from_c(ctypes.addressof(arr), arrow_schema))
-        return out
+        return (out, _bad_report(result_handle)) if with_bad else out
     finally:
         lib.rv_result_free(result_handle)
+
+
+# errors="raise" (the default): a record that does not decode fails the call.  errors="null": it becomes a row that is
+# null in every top-level column (Schema.permissive), and the call returns (batches, bad); `bad` lists the bad records
+# in record order: `record` (index in the call), `status` (rv_status) and `error` (the strict call's message).
+_BAD_SCHEMA = pa.schema([("record", pa.int64()), ("status", pa.int32()), ("error", pa.string())])
+
+
+def _permissive(errors) -> bool:
+    if errors == "raise":
+        return False
+    if errors == "null":
+        return True
+    raise ValueError(f"argument 'errors': expected \"raise\" or \"null\", got {errors!r}")
+
+
+def _bad_report(result_handle: int) -> pa.RecordBatch:
+    import numpy as np
+    n = lib.rv_result_num_bad(result_handle)
+    records = np.zeros(n, dtype=np.int64)
+    status = np.zeros(n, dtype=np.int32)
+    if n:
+        lib.rv_result_bad(result_handle, records.ctypes.data, status.ctypes.data, n)
+    text = [lib.rv_result_bad_message(result_handle, i).decode() for i in range(n)]
+    return pa.RecordBatch.from_arrays([pa.array(records), pa.array(status), pa.array(text, pa.string())], schema=_BAD_SCHEMA)
 
 
 _native_mod = None
@@ -322,21 +364,23 @@ class Framing(ctypes.Structure):
     _fields_ = [("header_bytes", ctypes.c_int32), ("check_magic", ctypes.c_int32), ("schema_id", ctypes.c_int64)]
 
 
-def _decode_list(records, schema: str, num_chunks: int, framing=None, columns=None, reader_schema=None) -> List[pa.RecordBatch]:
+def _decode_list(records, schema: str, num_chunks: int, framing=None, columns=None, reader_schema=None, errors="raise"):
+    permissive = _permissive(errors)
     if not isinstance(records, list):
         raise TypeError("argument 'list': expected a list of bytes")
-    s = _get_or_parse_schema(schema, columns, reader_schema)
+    s = _get_or_parse_schema(schema, columns, reader_schema, permissive)
     if framing is None:
         handle = _ext().decode_list(s.handle, records, int(num_chunks))
     else:
         handle = _ext().decode_list(s.handle, records, int(num_chunks), *framing)
-    return _export_batches(handle, s)
+    return _export_batches(handle, s, permissive)
 
 
 # Every decode entry point takes a keyword-only `columns`: a list of top-level field names.  The batches then hold only
 # those columns, in that order, each identical to that column of the full decode (Schema.project).
 # And a keyword-only `reader_schema`: the schema to read the data as (Schema.read_as); `schema` stays the schema the data
 # was written with.  With both, `columns` names the reader's fields.
+# The decodes of message lists and packed inputs also take a keyword-only `errors` ("raise" or "null", see _permissive).
 
 
 def deserialize_ocf(data, num_chunks=1, *, columns=None, reader_schema=None) -> List[pa.RecordBatch]:
@@ -362,26 +406,27 @@ def deserialize_ocf(data, num_chunks=1, *, columns=None, reader_schema=None) -> 
     return _export_batches(h.value, Schema._adopt(sh.value))
 
 
-def deserialize_confluent(list, schema, num_chunks=1, schema_id=None, *, columns=None, reader_schema=None):  # noqa: A002
+def deserialize_confluent(list, schema, num_chunks=1, schema_id=None, *, columns=None, reader_schema=None, errors="raise"):  # noqa: A002
     """list[bytes] of Confluent-framed Kafka messages (magic 0x00 + big-endian u32 schema id + Avro datum) ->
     `num_chunks` RecordBatches.  The 5-byte header is validated (the id too when `schema_id` is given) and skipped inside
     the decode kernel — no per-message slicing in Python (the reference expects callers to strip it, README.md:93-94)."""
     if num_chunks < 0:
         raise OverflowError("can't convert negative int to unsigned")
     return _decode_list(list, schema, num_chunks, framing=(5, 1, -1 if schema_id is None else int(schema_id)), columns=columns,
-                        reader_schema=reader_schema)
+                        reader_schema=reader_schema, errors=errors)
 
 
-def deserialize_single_object(list, schema, num_chunks=1, *, columns=None, reader_schema=None):  # noqa: A002
+def deserialize_single_object(list, schema, num_chunks=1, *, columns=None, reader_schema=None, errors="raise"):  # noqa: A002
     """list[bytes] of Avro single-object messages (C3 01 + the little-endian CRC-64-AVRO fingerprint of the writer schema
     + Avro datum) -> `num_chunks` RecordBatches.  Every header must name `schema`'s fingerprint (Schema.fingerprint); it is
     checked and skipped inside the decode kernel (rv_decode_host_single_object)."""
+    permissive = _permissive(errors)
     if num_chunks < 0:
         raise OverflowError("can't convert negative int to unsigned")
     if not isinstance(list, type([])):
         raise TypeError("argument 'list': expected a list of bytes")
-    s = _get_or_parse_schema(schema, columns, reader_schema)
-    return _export_batches(_ext().decode_list_single_object(s.handle, list, int(num_chunks)), s)
+    s = _get_or_parse_schema(schema, columns, reader_schema, permissive)
+    return _export_batches(_ext().decode_list_single_object(s.handle, list, int(num_chunks)), s, permissive)
 
 
 class Versions:
@@ -497,37 +542,41 @@ def last_versions_timings() -> dict:
     return dict(zip(("partition", "decodes", "take", "device"), buf))
 
 
-def deserialize_array(list, schema, *, columns=None, reader_schema=None):  # noqa: A002 - the reference names the parameter `list`
-    """list[bytes] of schemaless Avro datums -> one RecordBatch (src/lib.rs:56-71)."""
+def deserialize_array(list, schema, *, columns=None, reader_schema=None, errors="raise"):  # noqa: A002 - the reference names the parameter `list`
+    """list[bytes] of schemaless Avro datums -> one RecordBatch (src/lib.rs:56-71); errors="null": (batch, bad)."""
+    if _permissive(errors):
+        batches, bad = _decode_list(list, schema, 1, columns=columns, reader_schema=reader_schema, errors=errors)
+        return batches[0], bad
     return _decode_list(list, schema, 1, columns=columns, reader_schema=reader_schema)[0]
 
 
-def deserialize_array_threaded(list, schema, num_chunks, *, columns=None, reader_schema=None):  # noqa: A002
+def deserialize_array_threaded(list, schema, num_chunks, *, columns=None, reader_schema=None, errors="raise"):  # noqa: A002
     """list[bytes] -> `num_chunks` RecordBatches over contiguous row ranges (src/lib.rs:73-89;
     chunking per ruhvro/src/deserialize.rs:53-68)."""
     if num_chunks < 0:
         raise OverflowError("can't convert negative int to unsigned")  # usize extraction in PyO3
-    return _decode_list(list, schema, num_chunks, columns=columns, reader_schema=reader_schema)
+    return _decode_list(list, schema, num_chunks, columns=columns, reader_schema=reader_schema, errors=errors)
 
 
-def deserialize_array_threaded_spawn(list, schema, num_chunks, *, columns=None, reader_schema=None):  # noqa: A002
+def deserialize_array_threaded_spawn(list, schema, num_chunks, *, columns=None, reader_schema=None, errors="raise"):  # noqa: A002
     """Same results as deserialize_array_threaded (the reference only changes the tokio primitive,
     ruhvro/src/deserialize.rs:123-170)."""
-    return deserialize_array_threaded(list, schema, num_chunks, columns=columns, reader_schema=reader_schema)
+    return deserialize_array_threaded(list, schema, num_chunks, columns=columns, reader_schema=reader_schema, errors=errors)
 
 
 def decode_packed(data, offsets, n: int, schema: str, num_chunks: int = 1, framing: "Framing | None" = None, *,
-                  columns=None, reader_schema=None) -> List[pa.RecordBatch]:
+                  columns=None, reader_schema=None, errors="raise"):
     """Packed host buffers (numpy uint8 data + int64 offsets[n+1]) -> batches, through rv_decode_host (or
     rv_decode_host_framed when `framing` is given).  This is the C-ABI call a Rust/FFI caller makes; no Python list walk."""
     import numpy as np
-    s = _get_or_parse_schema(schema, columns, reader_schema)
+    permissive = _permissive(errors)
+    s = _get_or_parse_schema(schema, columns, reader_schema, permissive)
     data = np.ascontiguousarray(data, dtype=np.uint8)
     offsets = np.ascontiguousarray(offsets, dtype=np.int64)
     h = ctypes.c_void_p()
     _check(lib.rv_decode_host_framed(s.handle, data.ctypes.data if data.size else None, offsets.ctypes.data, n, num_chunks,
                                      ctypes.byref(framing) if framing is not None else None, ctypes.byref(h)))
-    return _export_batches(h.value, s)
+    return _export_batches(h.value, s, permissive)
 
 
 def _packed_view(arr):
@@ -554,7 +603,7 @@ def _packed_view(arr):
     return data, off.astype(np.int64, copy=False), n
 
 
-def deserialize_arrow_array(array, schema, num_chunks=1, *, columns=None, reader_schema=None):
+def deserialize_arrow_array(array, schema, num_chunks=1, *, columns=None, reader_schema=None, errors="raise"):
     """An Arrow Binary/LargeBinary array (or ChunkedArray) of schemaless datums -> `num_chunks` RecordBatches.
 
     The ingest shortcut of SURVEY §8(f) rank 2: what `per_datum_deserialize_threaded` builds internally at
@@ -562,8 +611,9 @@ def deserialize_arrow_array(array, schema, num_chunks=1, *, columns=None, reader
     list walk and no gather copy; results are identical to deserialize_array_threaded on `array.to_pylist()`."""
     if num_chunks < 0:
         raise OverflowError("can't convert negative int to unsigned")
+    _permissive(errors)
     data, off, n = _packed_view(array)
-    return decode_packed(data, off, n, schema, int(num_chunks), columns=columns, reader_schema=reader_schema)
+    return decode_packed(data, off, n, schema, int(num_chunks), columns=columns, reader_schema=reader_schema, errors=errors)
 
 
 def _encode(encode_fn, data, schema, *args) -> int:

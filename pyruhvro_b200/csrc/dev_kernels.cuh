@@ -287,7 +287,7 @@ __device__ __forceinline__ void prefetch_window(const DecodeParams& p, const Til
 // SM = true, the FAST flavour: returns != 0 when the record is not plain (dev_core.cuh) and reports nothing — the
 // caller repeats the record with the precise flavour.  SM = false, PRECISE: reports the record's first error and
 // returns its code.
-template <class W, bool SM>
+template <class W, bool SM, bool PERM = false>
 __device__ __forceinline__ uint32_t count_walk(const DecodeParams& p, const Tile& t, const SmemMap& m, const TileWindow& w, typename W::Cur& q) {
     WalkCtx<SM> c;
     const int64_t r = init_ctx(c, p, t, m, w);
@@ -300,7 +300,7 @@ __device__ __forceinline__ uint32_t count_walk(const DecodeParams& p, const Tile
 #if !defined(RV_ABL_NOCOUNTWALK)
     W::template walk<WM_COUNT>(c, p.n_nodes, q);
 #endif
-    if (!SM && c.in_range && c.err) report(p, r, c.err);
+    if (!SM && c.in_range && c.err && !(PERM && record_error(c.err))) report(p, r, c.err);
     return c.in_range ? c.err : 0u;
 }
 // Everything by value: a reference parameter of a function that is not inlined would force the caller's copy (the
@@ -312,6 +312,19 @@ __device__ __noinline__ CountOut<W> count_walk_global(const DecodeParams p, cons
     CountOut<W> o;
     o.err = count_walk<W, false>(p, t, m, w, o.q);
     return o;
+}
+// Permissive decodes: the same, except that a record error (record_error) is left to the caller instead of reported.
+template <class W>
+__device__ __noinline__ CountOut<W> count_walk_global_perm(const DecodeParams p, const Tile t, const SmemMap m, const TileWindow w) {
+    CountOut<W> o;
+    o.err = count_walk<W, false, true>(p, t, m, w, o.q);
+    return o;
+}
+
+template <class W, bool PERM>
+__device__ __forceinline__ CountOut<W> count_precise(const DecodeParams& p, const Tile& t, const SmemMap& m, const TileWindow& w) {
+    if constexpr (PERM) return count_walk_global_perm<W>(p, t, m, w);
+    else return count_walk_global<W>(p, t, m, w);
 }
 
 // ---- emit: staging map ------------------------------------------------------------------------
@@ -352,10 +365,14 @@ __device__ __forceinline__ void stage_map(const DecodeParams& p, const Tile& t, 
 
 // ---- emit -----------------------------------------------------------------------------------
 template <class W, bool SM>
-__device__ __forceinline__ void emit_walk(const DecodeParams& p, const Tile& t, const SmemMap& m, const TileWindow& w, typename W::Cur& q, const bool stage_on) {
+__device__ __forceinline__ void emit_walk(const DecodeParams& p, const Tile& t, const SmemMap& m, const TileWindow& w, typename W::Cur& q, const bool stage_on,
+                                          const uint32_t bad = 0u) {
     WalkCtx<SM> c;
     (void)init_ctx(c, p, t, m, w);
     c.stage_on = stage_on;
+    // permissive decodes: the count walk's verdict on a bad record.  Its row is emitted absent -- the walkers' top-level
+    // presence is false while c.err is set (interp.cuh; the permissive generated walker's vtop) -- and reads nothing.
+    if (bad) c.err = bad;
     const int tid = threadIdx.x;
     // offsets[0] = 0 of every offsets buffer of this chunk (first tile of the chunk only)
     if (t.local_tile == 0) {
@@ -378,6 +395,18 @@ __device__ __forceinline__ void emit_walk(const DecodeParams& p, const Tile& t, 
 template <class W>
 __device__ __noinline__ void emit_walk_global(const DecodeParams p, const Tile t, const SmemMap m, const TileWindow w, typename W::Cur q, const bool stage_on) {
     emit_walk<W, false>(p, t, m, w, q, stage_on);
+}
+template <class W>
+__device__ __noinline__ void emit_walk_global_perm(const DecodeParams p, const Tile t, const SmemMap m, const TileWindow w, typename W::Cur q, const bool stage_on,
+                                                   const uint32_t bad) {
+    emit_walk<W, false>(p, t, m, w, q, stage_on, bad);
+}
+
+template <class W, bool PERM>
+__device__ __forceinline__ void emit_precise(const DecodeParams& p, const Tile& t, const SmemMap& m, const TileWindow& w, typename W::Cur& q, const bool stage_on,
+                                             const uint32_t bad) {
+    if constexpr (PERM) emit_walk_global_perm<W>(p, t, m, w, q, stage_on, bad);
+    else { (void)bad; emit_walk_global<W>(p, t, m, w, q, stage_on); }
 }
 
 // Coalesced write-out of the staged Utf8 bytes, one warp per stream at a time.
@@ -413,7 +442,10 @@ __device__ __forceinline__ void stage_write_out(const DecodeParams& p, const Sme
 }
 
 // ---- the fused pass ---------------------------------------------------------------------------
-template <class W>
+// PERM (permissive decodes, rv_schema_permissive): a record with a record error (record_error) does not fail the call.
+// Its lane counts nothing, appends (record << 8 | code) to the bad-record list (bad_list_word) and emits its row absent
+// on the precise path; only the other codes (E_OVERFLOW, E_SCHEMA) are reported to CW_ERR and end the CTA's work.
+template <class W, bool PERM = false>
 __device__ __forceinline__ void fused_body(const DecodeParams& p, const int tile_id) {
     const Tile t = tile_of(p, tile_id);
     const SmemMap m = smem_map(p.n_nodes, p.n_streams, p.n_slots, p.smem_data_cap, p.smem_stage_cap, W::kRegCursors, W::kItemBytes);
@@ -432,15 +464,34 @@ __device__ __forceinline__ void fused_body(const DecodeParams& p, const int tile
         my_err = count_walk<W, true>(p, t, m, w, q);
         const bool not_plain = my_err != 0u;
         if (not_plain) {
-            const CountOut<W> o = count_walk_global<W>(p, t, m, w);
+            const CountOut<W> o = count_precise<W, PERM>(p, t, m, w);
             q = o.q;
             my_err = o.err;
         }
         warp_precise = __any_sync(0xFFFFFFFFu, not_plain);
     } else {
-        const CountOut<W> o = count_walk_global<W>(p, t, m, w);
+        const CountOut<W> o = count_precise<W, PERM>(p, t, m, w);
         q = o.q;
         my_err = o.err;
+    }
+    // A bad record (always settled by the precise walk above, so its warp emits with the precise walker too) counts
+    // nothing and is listed.  Every pass lists afresh: the host clears CW_BAD with the rest of the control block.
+    uint32_t bad = 0u;
+    if constexpr (PERM) {
+        if (my_err != 0u && record_error(my_err)) {
+            bad = my_err;
+            my_err = 0u;
+            if constexpr (W::kRegCursors) {
+#pragma unroll
+                for (int s = 0; s < W::kStreams; ++s) q.v[s] = 0;
+            } else {
+                uint32_t* cz = reinterpret_cast<uint32_t*>(rv_smem + m.cur);
+                for (int s = 0; s < p.n_streams; ++s) cz[s * kBlock + tid] = 0;
+            }
+            const unsigned long long* lw = p.ctrl + bad_list_word(p.k, p.n_streams);
+            const unsigned long long i = atomicAdd(p.ctrl + CW_BAD, 1ull);
+            if (i < lw[1]) reinterpret_cast<unsigned long long*>(lw[0])[i] = (static_cast<unsigned long long>(t.r0 + tid) << 8) | bad;
+        }
     }
 
     // ---- CTA-wide exclusive scan of every stream's lane counts.  One WARP scans one stream: each lane takes kBlock / 32
@@ -573,14 +624,14 @@ __device__ __forceinline__ void fused_body(const DecodeParams& p, const int tile
     const bool fast = w.staged && (flags[0] & 2u);
     if (fast) {
         if (!warp_precise) emit_walk<W, true>(p, t, m, w, q, true);
-        else emit_walk_global<W>(p, t, m, w, q, true);  // (warp-uniform) stages its strings like the other warps
+        else emit_precise<W, PERM>(p, t, m, w, q, true, bad);  // (warp-uniform) stages its strings like the other warps
         prefetch_window(p, w);
         if (p.n_utf8 > 0) stage_write_out(p, m);
     } else {
         // the tile's bytes or its strings do not fit shared memory: walk the records in global memory and write
         // strings straight to their Arrow buffers (slow; window sizing keeps such tiles rare)
         if (tid == 0) atomicAdd(p.ctrl + CW_SLOW_TILES, 1ull);
-        emit_walk_global<W>(p, t, m, w, q, false);
+        emit_precise<W, PERM>(p, t, m, w, q, false, bad);
     }
 }
 

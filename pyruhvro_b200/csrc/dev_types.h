@@ -110,6 +110,13 @@ enum ErrCode : uint32_t {
     E_VALUE = 11     // wider subset: a value its logical type cannot hold (uuid text that is not a UUID, decimal wider than 128 bits)
 };
 
+// Codes that belong to one record: a permissive decode turns such a record into a null row.  The rest (E_OVERFLOW: a
+// batch's offsets, malformed input offsets, a record of 4 GiB or more; E_SCHEMA) fail the call.
+#if defined(__CUDACC__)
+__host__ __device__
+#endif
+constexpr bool record_error(uint32_t code) { return code < 32u && ((0x387Eu >> code) & 1u) != 0u; }
+
 #ifndef RV_KBLOCK
 #define RV_KBLOCK 256
 #endif
@@ -131,8 +138,16 @@ enum CtrlWord : int {
     CW_SLOW_TILES = 4,  // tiles that did not fit shared memory and were walked in global memory
     CW_IN_FIRST = 5,    // offsets[0]
     CW_IN_LAST = 6,     // offsets[n]: the input's byte span sizes later calls' windows
+    CW_BAD = 7,         // permissive decodes: bad records listed (bad_list)
     CW_CHUNK_TOT = 8    // [k][n_streams] exact stream totals per chunk
 };
+// Permissive decodes (fused_body<W, true>) find their bad-record list in the two control words that follow the chunk
+// totals: its device address and its capacity.  Each bad record of the pass is one (record << 8 | code) entry, in no
+// order.  (A DecodeParams field would grow the strict kernel's by-value copies to its precise walkers and change its code.)
+#if defined(__CUDACC__)
+__host__ __device__
+#endif
+inline uint64_t bad_list_word(int k, int n_streams) { return uint64_t(CW_CHUNK_TOT) + uint64_t(k) * uint64_t(n_streams > 0 ? n_streams : 1); }
 
 // Kernel parameter block of the fused decode pass.
 struct DecodeParams {

@@ -612,6 +612,7 @@ using namespace rv;
 // Access to the schema internals lives in engine.cu.
 extern "C" const void* rv_schema_avro_root(const rv_schema* s);
 extern "C" int rv_schema_is_projection(const rv_schema* s);
+extern "C" int rv_schema_is_permissive(const rv_schema* s);
 extern "C" void rv_set_last_error(const char* msg);
 
 extern "C" const char* rv_internal_schema_json(const rv_schema* s, size_t* len);
@@ -979,6 +980,10 @@ static void for_each_group(int groups, const std::function<void(int)>& fn) {
 // chunks are the file's blocks).
 static rv_status encode_batch(const rv_schema* s, const ArrowArray* batch, const ArrowSchema* batch_schema, int64_t num_chunks, int out_kind,
                               uint64_t key, const OcfSpec* ocf, rv_encoded** out) {
+    if (rv_schema_is_permissive(s)) {
+        rv_set_last_error("fast_encode: a permissive handle (rv_schema_permissive) is not a schema to write with; encode with the full schema handle");
+        return RV_ERR_INVALID;
+    }
     if (rv_schema_is_projection(s)) {
         rv_set_last_error("fast_encode: a column projection (rv_schema_project) or a resolved handle (rv_schema_resolve) is not a schema to write with; encode with the full schema handle");
         return RV_ERR_INVALID;

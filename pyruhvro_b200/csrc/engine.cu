@@ -527,6 +527,10 @@ struct rv_result {
     std::vector<ChunkOut> chunks;
     std::vector<std::shared_ptr<Arena>> arenas;  // arenas[i] backs chunks[i] (one arena may back many chunks)
     int64_t arrow_bytes = 0;
+    // permissive decodes: the call's bad records in record order (record index in the call, the kernel's error code)
+    std::vector<int64_t> bad_records;
+    std::vector<uint32_t> bad_codes;
+    bool single_object = false;  // (the text of E_FRAME)
     ~rv_result() { if (schema) rv_schema_release(schema); }
 };
 
@@ -690,6 +694,19 @@ int64_t max_tile_span(const int64_t* offsets, int64_t n, int64_t k, int tile) {
         for (int64_t a = cs; a < ce; a += tile) mx = std::max(mx, offsets[std::min(a + tile, ce)] - offsets[a]);
     }
     return mx;
+}
+
+// A permissive pass's bad records (record << 8 | code) into record order.  The records are distinct and below n: an LSD
+// radix sort on them, 11 bits a pass (std::sort took 12 ms for 100 000 entries on the build host).
+void sort_bad_words(std::vector<unsigned long long>& w, int64_t n) {
+    std::vector<unsigned long long> tmp(w.size());
+    for (int shift = 8; (static_cast<unsigned long long>(n) << 8) >> shift != 0; shift += 11) {
+        size_t count[2049] = {};
+        for (unsigned long long x : w) ++count[((x >> shift) & 2047u) + 1];
+        for (int d = 0; d < 2048; ++d) count[d + 1] += count[d];
+        for (unsigned long long x : w) tmp[count[(x >> shift) & 2047u]++] = x;
+        w.swap(tmp);
+    }
 }
 
 // ---- the decode call ------------------------------------------------------------------------
@@ -884,7 +901,7 @@ rv_status decode_on_device(rv_schema* s, const uint8_t* d_data, const int64_t* d
     // ---- per-call device state: [ctrl][bufs table][caps][null-count jobs][ones] in ONE block, initialised by one
     // copy from a pinned template and (ctrl + ones) read back by one copy ------------------------------------
     const int nv = int(plan.validity_slots.size());
-    const size_t ctrl_words = size_t(CW_CHUNK_TOT) + chunk_tot.size();
+    const size_t ctrl_words = size_t(CW_CHUNK_TOT) + chunk_tot.size() + (plan.permissive ? 2 : 0);  // (+ the bad-record list's words)
     const size_t off_ctrl = 0;
     const size_t off_ones = align_up(off_ctrl + ctrl_words * 8, 16);
     const size_t ones_n = size_t(k) * size_t(std::max(nv, 1));
@@ -896,9 +913,10 @@ rv_status decode_on_device(rv_schema* s, const uint8_t* d_data, const int64_t* d
     uint8_t* h_misc = t_scratch.get(misc_bytes + back_bytes);
     if (!h_misc) return fail(RV_ERR_CUDA, "pinned allocation of the call state failed");
     uint8_t* h_back = h_misc + misc_bytes;
-    DevBuf d_misc, d_state;
+    DevBuf d_misc, d_state, d_bad;
     RV_CUDA(d_misc.alloc(misc_bytes, stream));
     RV_CUDA(d_state.alloc(size_t(Sx) * size_t(n_tiles) * 8, stream));
+    if (plan.permissive) RV_CUDA(d_bad.alloc(size_t(n) * 8, stream));  // room for every record: a pass lists each bad record once
     SyncOnExit guard{stream};  // declared after the cached device blocks: runs before they go back to the cache
     uint8_t* dm = static_cast<uint8_t*>(d_misc.p);
     p.ctrl = reinterpret_cast<unsigned long long*>(dm + off_ctrl);
@@ -963,6 +981,10 @@ rv_status decode_on_device(rv_schema* s, const uint8_t* d_data, const int64_t* d
         hc[CW_ERR] = ~0ull;
         hc[CW_MAX_SPAN] = stats.tile == tile ? stats.max_span : 0ull;   // the kernel only raises these
         hc[CW_MAX_UTF8] = stats.tile == tile ? stats.max_utf8 : 0ull;
+        if (plan.permissive) {
+            hc[bad_list_word(k, S)] = static_cast<unsigned long long>(reinterpret_cast<uintptr_t>(d_bad.p));
+            hc[bad_list_word(k, S) + 1] = static_cast<unsigned long long>(n);
+        }
         if (!count_only) {
             void** hb = reinterpret_cast<void**>(h_misc + off_bufs);
             for (int j = 0; j < k; ++j)
@@ -1005,7 +1027,7 @@ rv_status decode_on_device(rv_schema* s, const uint8_t* d_data, const int64_t* d
                 return decode_on_device(s, d_data, d_offsets, n, num_chunks, hints, stream, device, out, record_base, err_word_out);
             }
         } else {
-            launch_fused(p, smem_bytes, stream);
+            launch_fused(p, smem_bytes, stream, plan.permissive);
         }
         RV_CUDA(cudaEventRecord(ev[1], stream));
         t_launches += 1;
@@ -1064,6 +1086,20 @@ rv_status decode_on_device(rv_schema* s, const uint8_t* d_data, const int64_t* d
         caps = chunk_tot;
         exact_caps = true;
         count_only = false;
+    }
+
+    // ---- the bad records of a permissive call: read back only when there are some (a clean call keeps its one
+    // synchronisation); the kernel lists them in completion order
+    res->single_object = hints.single_object;
+    if (const unsigned long long nbad = hb_ctrl[CW_BAD]) {
+        if (nbad > static_cast<unsigned long long>(n)) return fail(RV_ERR_CUDA, "internal error: more bad records than records");
+        std::vector<unsigned long long> words(static_cast<size_t>(nbad));
+        RV_CUDA(cudaMemcpy(words.data(), d_bad.p, words.size() * 8, cudaMemcpyDeviceToHost));
+        sort_bad_words(words, n);
+        for (unsigned long long w : words) {
+            res->bad_records.push_back(int64_t(w >> 8) + record_base);
+            res->bad_codes.push_back(uint32_t(w & 0xFF));
+        }
     }
 
     // ---- exact logical sizes on top of the capacity-planned placement ---------------------------
@@ -1187,6 +1223,7 @@ rv_status rv_schema_project(const rv_schema* s, const char* const* columns, int6
             p->fields.push_back(s->fields[size_t(i)]);
         }
         p->plan = p->res ? build_resolved_plan(*p->res, all, &p->keep) : build_plan(*p->avro, all, &p->keep);
+        p->plan.permissive = s->plan.permissive;
         p->has_plan = true;
         *out = p.release();
         return RV_OK;
@@ -1223,6 +1260,39 @@ rv_status rv_schema_resolve(const rv_schema* writer, const rv_schema* reader, rv
         return fail(RV_ERR_SCHEMA, e.what());
     }
 }
+
+rv_status rv_schema_permissive(const rv_schema* s, rv_schema** out) {
+    if (!s || !out) return fail(RV_ERR_INVALID, "null argument");
+    *out = nullptr;
+    if (s->plan.permissive) return fail(RV_ERR_INVALID, "rv_schema_permissive: the handle is already permissive");
+    rv_status st = check_decodable(s);
+    if (st) return st;
+    try {
+        // R': the handle's output schema with every top-level field optional, read from the writer by the resolution rules
+        // (a writer T read as a reader ["null", T] gets a validity bitmap and reads no branch)
+        auto p = std::make_unique<rv_schema>();
+        p->avro = s->avro;
+        p->json = s->json;
+        p->canonical = s->canonical; p->canonical_why = s->canonical_why; p->fingerprint = s->fingerprint;
+        p->reader = std::shared_ptr<const AvroNode>(optional_fields(s->res ? *s->reader : *s->avro).release());
+        p->res = std::make_shared<const Resolution>(resolve_schemas(*p->avro, *p->reader));
+        p->supported = true;
+        p->has_fields = true;
+        p->keep = s->keep;
+        const std::vector<ArrowField> all = to_arrow_fields(*p->reader);
+        if (p->keep.empty()) p->fields = all;
+        else for (int i : p->keep) p->fields.push_back(all[size_t(i)]);
+        p->plan = build_resolved_plan(*p->res, all, p->keep.empty() ? nullptr : &p->keep);
+        p->plan.permissive = true;
+        p->has_plan = true;
+        *out = p.release();
+        return RV_OK;
+    } catch (const std::exception& e) {
+        return fail(RV_ERR_SCHEMA, e.what());
+    }
+}
+
+int rv_schema_is_permissive(const rv_schema* s) { return s && s->plan.permissive ? 1 : 0; }
 
 int64_t rv_schema_canonical_form(const rv_schema* s, char* buf, size_t cap) {
     if (!s) { fail(RV_ERR_INVALID, "null argument"); return -1; }
@@ -1879,6 +1949,10 @@ static rv_status decode_host_call(rv_schema* s, const uint8_t* data, const int64
             res->chunks.push_back(std::move(part->chunks[0]));
             res->arenas.push_back(part->arenas[0]);
             res->arrow_bytes += part->arrow_bytes;
+            // (each chunk listed call-global record indices in order; chunks come in record order)
+            res->bad_records.insert(res->bad_records.end(), part->bad_records.begin(), part->bad_records.end());
+            res->bad_codes.insert(res->bad_codes.end(), part->bad_codes.begin(), part->bad_codes.end());
+            res->single_object = part->single_object;
         }
         rv_result_free(part);
     }
@@ -1893,6 +1967,21 @@ int64_t rv_result_num_rows(const rv_result* r, int64_t batch) {
     return r->chunks[size_t(batch)].rows;
 }
 int64_t rv_result_arrow_bytes(const rv_result* r) { return r ? r->arrow_bytes : 0; }
+int64_t rv_result_num_bad(const rv_result* r) { return r ? int64_t(r->bad_records.size()) : 0; }
+int64_t rv_result_bad(const rv_result* r, int64_t* records, int32_t* status, int64_t cap) {
+    if (!r || cap < 0 || (cap > 0 && (!records || !status))) { fail(RV_ERR_INVALID, "null argument"); return -1; }
+    const int64_t n = std::min<int64_t>(cap, int64_t(r->bad_records.size()));
+    for (int64_t i = 0; i < n; ++i) {
+        records[i] = r->bad_records[size_t(i)];
+        status[i] = int32_t(status_of(r->bad_codes[size_t(i)]));
+    }
+    return int64_t(r->bad_records.size());
+}
+const char* rv_result_bad_message(const rv_result* r, int64_t i) {
+    if (!r || i < 0 || i >= int64_t(r->bad_codes.size())) return nullptr;
+    const uint32_t code = r->bad_codes[size_t(i)];
+    return code == E_FRAME && r->single_object ? kSingleObjectFrameText : err_text(code);
+}
 int64_t rv_result_buffer_bytes(const rv_result* r) {
     if (!r) return 0;
     int64_t total = 0;
@@ -2300,6 +2389,13 @@ rv_status check_versions_input(const rv_versions* v, int64_t n, bool have_ptrs, 
     return RV_OK;
 }
 
+bool permissive_in(const rv_schema* reader, const rv_schema* const* writers, int64_t n_writers) {
+    if (reader && reader->plan.permissive) return true;
+    for (int64_t i = 0; writers && i < n_writers; ++i)
+        if (writers[i] && writers[i]->plan.permissive) return true;
+    return false;
+}
+
 // The writers of `v` (its keys already in place, in `order`) resolved to the reader and projected to `columns`.
 rv_status register_writers(const rv_schema* reader, const rv_schema* const* writers, const std::vector<size_t>& order,
                            const char* const* columns, int64_t n_columns, std::unique_ptr<rv_versions> v, rv_versions** out) {
@@ -2348,6 +2444,8 @@ rv_status rv_versions_create(const rv_schema* reader, const int64_t* schema_ids,
     if (n_writers < 1) return fail(RV_ERR_INVALID, "schema versions: no writer schemas");
     if (n_writers > kMaxVersions) return fail(RV_ERR_INVALID, "schema versions: more than " + std::to_string(kMaxVersions) + " writer schemas");
     auto bad_handle = [](const rv_schema* s) { return !s || !s->keep.empty() || s->res; };
+    if (permissive_in(reader, writers, n_writers))
+        return fail(RV_ERR_INVALID, "schema versions: a permissive handle (rv_schema_permissive) cannot be registered; bad rows are not supported here");
     if (bad_handle(reader)) return fail(RV_ERR_INVALID, "schema versions: pass the handle of the reader's full schema (rv_schema_parse)");
     std::vector<size_t> order(static_cast<size_t>(n_writers));
     for (int64_t i = 0; i < n_writers; ++i) {
@@ -2375,6 +2473,8 @@ rv_status rv_versions_create_single_object(const rv_schema* reader, const rv_sch
     if (n_writers < 1) return fail(RV_ERR_INVALID, "schema versions: no writer schemas");
     if (n_writers > kMaxVersions) return fail(RV_ERR_INVALID, "schema versions: more than " + std::to_string(kMaxVersions) + " writer schemas");
     auto bad_handle = [](const rv_schema* s) { return !s || !s->keep.empty() || s->res; };
+    if (permissive_in(reader, writers, n_writers))
+        return fail(RV_ERR_INVALID, "schema versions: a permissive handle (rv_schema_permissive) cannot be registered; bad rows are not supported here");
     if (bad_handle(reader)) return fail(RV_ERR_INVALID, "schema versions: pass the handle of the reader's full schema (rv_schema_parse)");
     std::vector<size_t> order(static_cast<size_t>(n_writers));
     for (int64_t i = 0; i < n_writers; ++i) {

@@ -172,11 +172,13 @@ void launch_concat_bits(uint32_t* dst, long long dst_bit, const uint32_t* src, l
 cudaError_t prepare_kernels() {
     cudaError_t e = cudaFuncSetAttribute(fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(fused_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
+    if (e == cudaSuccess) e = prepare_kernels_permissive();
     return e;
 }
 
-void launch_fused(const DecodeParams& p, size_t smem, cudaStream_t s) {
-    fused_kernel<<<unsigned(p.n_tiles), kBlock, smem, s>>>(p);
+void launch_fused(const DecodeParams& p, size_t smem, cudaStream_t s, bool permissive) {
+    if (permissive) launch_fused_permissive(p, smem, s);
+    else fused_kernel<<<unsigned(p.n_tiles), kBlock, smem, s>>>(p);
 }
 
 void launch_null_count(const NullCountJob* jobs, int n_jobs, long long* out, cudaStream_t s) {

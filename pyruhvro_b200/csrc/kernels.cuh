@@ -33,7 +33,10 @@ struct PushJob {
 
 cudaError_t prepare_kernels();  // opt in to large dynamic shared memory (once per device)
 
-void launch_fused(const DecodeParams& p, size_t smem, cudaStream_t s);   // interpreter walker, one CTA per tile
+void launch_fused(const DecodeParams& p, size_t smem, cudaStream_t s, bool permissive = false);  // interpreter walker, one CTA per tile
+// the permissive instance (kernels_perm.cu, a translation unit of its own so that the two compile side by side)
+cudaError_t prepare_kernels_permissive();
+void launch_fused_permissive(const DecodeParams& p, size_t smem, cudaStream_t s);
 void launch_rebase_i32(int32_t* dst, const int32_t* src, long long n, int32_t add, cudaStream_t s);
 void launch_concat_bits(uint32_t* dst, long long dst_bit, const uint32_t* src, long long nbits, cudaStream_t s);
 void launch_null_count(const NullCountJob* jobs, int n_jobs, long long* out, cudaStream_t s);

@@ -64,6 +64,8 @@ struct Plan {
     std::vector<int> validity_slots; // slots with role Validity (null counts are computed for these)
     int n_spaces = 1;
     int max_depth = 0;
+    // rv_schema_permissive: bad records become null rows (the fused kernel's permissive instance, dev_kernels.cuh)
+    bool permissive = false;
 };
 
 // Throws std::runtime_error when the schema exceeds a documented limit.

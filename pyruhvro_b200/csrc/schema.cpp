@@ -840,6 +840,22 @@ Resolution resolve_schemas(const AvroNode& writer, const AvroNode& reader) {
     return resolve_node(writer, reader, std::string());
 }
 
+std::unique_ptr<AvroNode> optional_fields(const AvroNode& top) {
+    if (top.k != AK::Record) throw std::runtime_error("a permissive decode needs a record schema");
+    auto r = clone_node(top);
+    for (AvroField& f : r->fields) {
+        // (a map stays as it is: ["null", map] has no Arrow form here, as in the reference's schema_translate)
+        if (f.type->k == AK::Union || f.type->k == AK::Null || f.type->k == AK::Map) continue;
+        auto u = mk(AK::Union);
+        const bool value_default = f.dflt && f.dflt->kind != Json::Null;
+        if (value_default) u->sub.push_back(std::move(f.type));
+        u->sub.push_back(mk(AK::Null));
+        if (!value_default) u->sub.push_back(std::move(f.type));
+        f.type = std::move(u);
+    }
+    return r;
+}
+
 // ---- Parsing Canonical Form and CRC-64-AVRO (the specification's "Schema Fingerprints") -------------------------------
 namespace {
 

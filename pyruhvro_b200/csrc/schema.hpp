@@ -106,6 +106,12 @@ struct Resolution {
 // and the host emulation both build from it.
 Resolution resolve_schemas(const AvroNode& writer, const AvroNode& reader);
 
+// The reader schema of a permissive decode (rv_schema_permissive): the record `top` with every top-level field whose type
+// is not a union, null or a map made optional, T -> ["null", T].  A field with a non-null default becomes [T, "null"]
+// instead, where the default stays valid (a union's default belongs to its first branch); both are the same Arrow column.
+// A map stays as it is: a nullable map has no Arrow form here (to_arrow_fields refuses ["null", map], as the reference does).
+std::unique_ptr<AvroNode> optional_fields(const AvroNode& top);
+
 // ---- schema fingerprints (the specification's "Parsing Canonical Form" and "Schema Fingerprints") --------------------
 // The canonical form of a parsed schema: primitives as bare names, named types by fullname (written in full at their
 // first occurrence, by fullname after that), only name / type / fields / symbols / items / values / size in that order,

@@ -42,12 +42,24 @@ def schemas():
     out += [BIG_SCHEMA, BOOL_STR_SCHEMA, ZW_SCHEMA]
     from tests.test_resolve_edges import JIT_RESOLVED
     out += JIT_RESOLVED  # a resolved plan (writer, reader) has its own walker
+    from tests.test_gpu_permissive import jit_permissive
+    out += [("permissive",) + item for item in jit_permissive()]  # so has a permissive one (schema, columns, reader)
     return list(dict.fromkeys(out))
 
 
 def one(item):
-    """A schema, (schema, columns) for a projected plan or (writer, reader) for a resolved one."""
+    """A schema, (schema, columns) for a projected plan, (writer, reader) for a resolved one or ("permissive", schema,
+    columns, reader) for a permissive one."""
     import pyruhvro_b200 as pr
+    if isinstance(item, tuple) and item[0] == "permissive":
+        _, sj, cols, reader = item
+        s = pr.Schema(sj)
+        if reader is not None:
+            s = s.read_as(reader)
+        if cols is not None:
+            s = s.project(list(cols))
+        s.permissive().precompile("sm_90a")
+        return 1
     sj, cols = item if isinstance(item, tuple) else (item, None)
     s = pr.Schema(sj)
     if isinstance(cols, str):
