@@ -229,6 +229,17 @@ void rv_versions_release(rv_versions* v);
  * a writer that does not resolve to the reader. */
 rv_status rv_versions_create_single_object(const rv_schema* reader, const rv_schema* const* writers, int64_t n_writers,
                                            const char* const* columns, int64_t n_columns, rv_versions** out);
+/* A permissive registry made from `v`: same keys, writers and columns; its batches are R' (rv_schema_permissive of the
+ * reader, projected to the columns), and rv_decode_*_versions with it turns a bad message into a null row and reports
+ * it (rv_result_num_bad / rv_result_bad / rv_result_bad_message) instead of failing the call.  A message is bad when
+ * the strict decode of it alone, with `v`, fails with a framing error (short, wrong magic byte, or a schema id or
+ * fingerprint that is not registered: RV_ERR_FRAME, whose message names the id or fingerprint) or a record error of its
+ * writer's resolved decode (RV_ERR_EOF, _VARINT, _BOOL, _NEG_LEN, _BRANCH, _ENUM including an unmapped symbol, _VALUE).
+ * Its row is what a permissive decode writes for a bad record: null in every top-level column, an empty map in a map
+ * column, type id 0 with absent children in an N-variant union column.  The report is in message order; each message is
+ * the strict one without "(record N)".  RV_ERR_OVERFLOW, RV_ERR_SCHEMA, RV_ERR_INVALID and RV_ERR_CUDA still fail the
+ * call.  `v` is unchanged and independent of the result.  RV_ERR_INVALID: `v` is already permissive. */
+rv_status rv_versions_permissive(const rv_versions* v, rv_versions** out);
 
 /* n Confluent messages (0x00, the big-endian u32 schema id, the datum) -- or, for a single-object registry, n
  * single-object messages (C3 01, the writer's fingerprint, the datum) -- -> num_chunks batches in the reader's Arrow form

@@ -91,6 +91,7 @@ def _bind(L):
     L.rv_decode_ocf_host_resolved.argtypes = [vp, i64, i64, vp, vp, i64, ctypes.POINTER(vp), ctypes.POINTER(vp)]
     L.rv_versions_create.argtypes = [vp, vp, vp, i64, vp, i64, ctypes.POINTER(vp)]
     L.rv_versions_create_single_object.argtypes = [vp, vp, i64, vp, i64, ctypes.POINTER(vp)]
+    L.rv_versions_permissive.argtypes = [vp, ctypes.POINTER(vp)]
     L.rv_versions_release.argtypes = [vp]
     L.rv_versions_release.restype = None
     L.rv_decode_host_versions.argtypes = [vp, vp, vp, i64, i64, ctypes.POINTER(vp)]
@@ -466,6 +467,18 @@ class Versions:
         _check(lib.rv_versions_create(full.handle, ids, hs, n, names, len(keep), ctypes.byref(h)))
         self.handle = h.value
 
+    def permissive(self) -> "Versions":
+        """A registry whose decodes turn a bad message into a null row and report it (rv_versions_permissive): a damaged
+        datum, a short message, a wrong magic byte, or a schema id or fingerprint this registry does not know.  Its
+        batches are the reader's with the top-level fields made nullable, as Schema.permissive makes them."""
+        h = ctypes.c_void_p()
+        _check(lib.rv_versions_permissive(self.handle, ctypes.byref(h)))
+        p = Versions.__new__(Versions)
+        p.handle = h.value
+        p.reader = self.reader.permissive()
+        p._writers = self._writers
+        return p
+
     def __del__(self):
         h, self.handle = getattr(self, "handle", None), None
         if h:
@@ -475,7 +488,18 @@ class Versions:
 _versions_cache = {}
 
 
-def _get_or_create_versions(writer_schemas, reader_schema, columns) -> Versions:
+def _cached_versions(key, make, permissive: bool) -> Versions:
+    """The registry of `key` (made by make() once), or its permissive form, cached under the mode too."""
+    with _schema_lock:
+        v = _versions_cache.get(key + (permissive,))
+    if v is not None:
+        return v
+    v = _cached_versions(key, make, False).permissive() if permissive else make()
+    with _schema_lock:
+        return _versions_cache.setdefault(key + (permissive,), v)
+
+
+def _get_or_create_versions(writer_schemas, reader_schema, columns, permissive=False) -> Versions:
     if not isinstance(writer_schemas, dict):
         raise TypeError("argument 'writer_schemas': expected a dict[int, str]")
     if not isinstance(reader_schema, str):
@@ -485,34 +509,33 @@ def _get_or_create_versions(writer_schemas, reader_schema, columns) -> Versions:
             raise TypeError("argument 'columns': expected a list of field names, not a single string")
         columns = tuple(columns)
     key = (tuple(sorted(writer_schemas.items())), reader_schema, columns)
-    with _schema_lock:
-        v = _versions_cache.get(key)
-    if v is not None:
-        return v
-    v = Versions(writer_schemas, reader_schema, columns)
-    with _schema_lock:
-        return _versions_cache.setdefault(key, v)
+    return _cached_versions(key, lambda: Versions(writer_schemas, reader_schema, columns), permissive)
 
 
-def deserialize_confluent_versions(list, writer_schemas, reader_schema, num_chunks=1, *, columns=None):  # noqa: A002
+def deserialize_confluent_versions(list, writer_schemas, reader_schema, num_chunks=1, *, columns=None, errors="raise"):  # noqa: A002
     """list[bytes] of Confluent-framed Kafka messages written with several schema versions -> `num_chunks` RecordBatches
     in `reader_schema`'s Arrow form, rows in message order.  `writer_schemas` maps every schema id that may occur to the
     writer schema it names (dict[int, str]); each message is decoded with its own writer's schema and resolved to the
-    reader (rv_decode_host_versions).  An id outside the map is an error, like a short message or a wrong magic byte."""
+    reader (rv_decode_host_versions).  An id outside the map is an error, like a short message or a wrong magic byte.
+    errors="null": such a message, and one whose datum does not decode, becomes a null row instead (Versions.permissive),
+    and the call returns (batches, bad) as the other decodes do; an unregistered id is reported with its id."""
+    permissive = _permissive(errors)
     if num_chunks < 0:
         raise OverflowError("can't convert negative int to unsigned")
     if not isinstance(list, type([])):
         raise TypeError("argument 'list': expected a list of bytes")
-    v = _get_or_create_versions(writer_schemas, reader_schema, columns)
-    return _export_batches(_ext().decode_list_versions(v.handle, list, int(num_chunks)), v.reader)
+    v = _get_or_create_versions(writer_schemas, reader_schema, columns, permissive)
+    return _export_batches(_ext().decode_list_versions(v.handle, list, int(num_chunks)), v.reader, permissive)
 
 
-def deserialize_single_object_versions(list, writer_schemas, reader_schema, num_chunks=1, *, columns=None):  # noqa: A002
+def deserialize_single_object_versions(list, writer_schemas, reader_schema, num_chunks=1, *, columns=None, errors="raise"):  # noqa: A002
     """list[bytes] of Avro single-object messages written with several schemas -> `num_chunks` RecordBatches in
     `reader_schema`'s Arrow form, rows in message order.  `writer_schemas` (list[str]) holds every writer schema that may
     occur; each message is decoded with the writer whose fingerprint its header names and resolved to the reader
     (rv_decode_host_versions).  An unregistered fingerprint is an error, like a short message or a wrong C3 01 marker.
-    Two writers with the same canonical form cannot be told apart on the wire and are refused."""
+    Two writers with the same canonical form cannot be told apart on the wire and are refused.  errors="null": as in
+    deserialize_confluent_versions, an unregistered fingerprint is reported with its fingerprint."""
+    permissive = _permissive(errors)
     if num_chunks < 0:
         raise OverflowError("can't convert negative int to unsigned")
     if not isinstance(list, type([])):
@@ -526,13 +549,8 @@ def deserialize_single_object_versions(list, writer_schemas, reader_schema, num_
             raise TypeError("argument 'columns': expected a list of field names, not a single string")
         columns = tuple(columns)
     key = ("single_object", tuple(writer_schemas), reader_schema, columns)
-    with _schema_lock:
-        v = _versions_cache.get(key)
-    if v is None:
-        v = Versions(writer_schemas, reader_schema, columns, single_object=True)
-        with _schema_lock:
-            v = _versions_cache.setdefault(key, v)
-    return _export_batches(_ext().decode_list_versions(v.handle, list, int(num_chunks)), v.reader)
+    v = _cached_versions(key, lambda: Versions(writer_schemas, reader_schema, columns, single_object=True), permissive)
+    return _export_batches(_ext().decode_list_versions(v.handle, list, int(num_chunks)), v.reader, permissive)
 
 
 def last_versions_timings() -> dict:

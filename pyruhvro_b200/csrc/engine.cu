@@ -530,6 +530,7 @@ struct rv_result {
     // permissive decodes: the call's bad records in record order (record index in the call, the kernel's error code)
     std::vector<int64_t> bad_records;
     std::vector<uint32_t> bad_codes;
+    std::vector<std::string> bad_texts;  // each bad record's message when it names the record's own header (permissive registries)
     bool single_object = false;  // (the text of E_FRAME)
     ~rv_result() { if (schema) rv_schema_release(schema); }
 };
@@ -1979,6 +1980,7 @@ int64_t rv_result_bad(const rv_result* r, int64_t* records, int32_t* status, int
 }
 const char* rv_result_bad_message(const rv_result* r, int64_t i) {
     if (!r || i < 0 || i >= int64_t(r->bad_codes.size())) return nullptr;
+    if (!r->bad_texts.empty()) return r->bad_texts[size_t(i)].c_str();
     const uint32_t code = r->bad_codes[size_t(i)];
     return code == E_FRAME && r->single_object ? kSingleObjectFrameText : err_text(code);
 }
@@ -2150,6 +2152,7 @@ struct rv_versions {
     std::vector<uint64_t> fps;            // single-object: the writers' CRC-64-AVRO fingerprints, ascending
     std::vector<rv_schema*> writers;      // the resolved (and projected) handle of ids[i] / fps[i]
     std::vector<VersionPairing> pairs;    // writers[i]'s plan next to the reader's
+    bool permissive = false;              // rv_versions_permissive: reader and writers are permissive handles
     ~rv_versions() {
         rv_schema_release(reader);
         for (rv_schema* w : writers) rv_schema_release(w);
@@ -2164,6 +2167,17 @@ std::string hex_fingerprint(uint64_t fp) {
     char b[24];
     std::snprintf(b, sizeof b, "0x%016llx", static_cast<unsigned long long>(fp));
     return b;
+}
+
+// The message of an E_FRAME_ID message whose header is `hdr`: its schema id or fingerprint is not registered.
+std::string unregistered_text(const rv_versions* v, const uint8_t* hdr) {
+    if (v->single_object) {
+        uint64_t fp = 0;
+        for (int b = 0; b < 8; ++b) fp |= uint64_t(hdr[2 + b]) << (8 * b);
+        return "single-object message: schema fingerprint " + hex_fingerprint(fp) + " is not registered";
+    }
+    const uint32_t id = (uint32_t(hdr[1]) << 24) | (uint32_t(hdr[2]) << 16) | (uint32_t(hdr[3]) << 8) | uint32_t(hdr[4]);
+    return "framed message: schema id " + std::to_string(id) + " is not registered";
 }
 
 // The framing of writer w's messages: its Confluent header, or its single-object header.
@@ -2197,6 +2211,8 @@ rv_status decode_versions(const rv_versions* v, const uint8_t* d_data, const int
     for (float& t : t_vtimings) t = 0;
     if (n == 0) return decode_on_device(v->reader, nullptr, nullptr, 0, num_chunks, InputHints{}, stream, device, out);
     const int W = int(v->writers.size());
+    const bool perm = v->permissive;
+    const int W1 = perm ? W + 1 : W;  // table columns: a permissive registry's last is every chunk's bad group (writer W)
     const int64_t k64 = clamp_chunks(num_chunks, n);
     if (k64 > (int64_t(1) << 24)) return fail(RV_ERR_INVALID, "num_chunks above 2^24 is not supported");
     const int k = int(k64);
@@ -2204,18 +2220,19 @@ rv_status decode_versions(const rv_versions* v, const uint8_t* d_data, const int
     const int64_t tpc = std::max<int64_t>(1, (chunk_rows + kTakeBlock - 1) / kTakeBlock);
     const int64_t n_tiles = tpc * (k - 1) + (last_rows + kTakeBlock - 1) / kTakeBlock;
     if (n_tiles > 0x7FFFFFF0ll || n >= (int64_t(1) << 40)) return fail(RV_ERR_INVALID, "too many records for one call");
-    const size_t G = size_t(k) * size_t(W);
+    const size_t G = size_t(k) * size_t(W1);
     cudaEvent_t* ev = nullptr;
     RV_CUDA(t_vevents.get(device, &ev));
 
-    // ---- partition: count + scan, one read-back of the group sizes and the framing errors
+    // ---- partition: count + scan, one read-back of the group sizes, the framing errors and the bad-group list's count
     size_t off = 0;
     auto take_off = [&](size_t bytes) { const size_t o = off; off = align_up(off + bytes, 16); return o; };
-    const size_t o_ids = take_off(size_t(W) * 8), o_err = take_off(8 + G * 16), o_tot = o_err + 8, o_cnt = take_off(size_t(n_tiles) * W * 4),
-                 o_bytes = take_off(size_t(n_tiles) * W * 8), o_msgw = take_off(size_t(n) * 2), o_map0 = take_off(size_t(n) * 8),
-                 o_gdata = take_off(G * 8), o_goff = take_off(G * 8);
-    DevBuf d_part, d_gdata, d_goffs, d_take;
+    const size_t o_ids = take_off(size_t(W) * 8), o_err = take_off(16 + G * 16), o_nbad = o_err + 8, o_tot = o_err + 16,
+                 o_cnt = take_off(size_t(n_tiles) * W1 * 4), o_bytes = take_off(size_t(n_tiles) * W1 * 8), o_msgw = take_off(size_t(n) * 2),
+                 o_map0 = take_off(size_t(n) * 8), o_gdata = take_off(G * 8), o_goff = take_off(G * 8);
+    DevBuf d_part, d_gdata, d_goffs, d_take, d_bad, d_inv, d_hdr;
     RV_CUDA(d_part.alloc(off, stream));
+    if (perm) RV_CUDA(d_bad.alloc(size_t(n) * 8, stream));  // every message is listed at most once, by the partition or a sub-decode
     SyncOnExit guard{stream};  // declared after the cached device blocks: runs before they go back to the cache
     uint8_t* dp = static_cast<uint8_t*>(d_part.p);
     std::vector<uint32_t> ids32(v->ids.begin(), v->ids.end());
@@ -2223,7 +2240,7 @@ rv_status decode_versions(const rv_versions* v, const uint8_t* d_data, const int
     const size_t key_bytes = v->single_object ? v->fps.size() * 8 : ids32.size() * 4;
     VersionsParams p{};
     p.data = d_data; p.offsets = d_offsets; p.n = n; p.chunk_rows = chunk_rows;
-    p.k = k; p.tiles_per_chunk = int32_t(tpc); p.n_tiles = int32_t(n_tiles); p.n_ids = W;
+    p.k = k; p.tiles_per_chunk = int32_t(tpc); p.n_tiles = int32_t(n_tiles); p.n_ids = W1;
     p.ids = reinterpret_cast<const uint32_t*>(dp + o_ids);
     p.fps = reinterpret_cast<const unsigned long long*>(dp + o_ids);
     p.err = reinterpret_cast<unsigned long long*>(dp + o_err);
@@ -2234,24 +2251,30 @@ rv_status decode_versions(const rv_versions* v, const uint8_t* d_data, const int
     p.map0 = reinterpret_cast<unsigned long long*>(dp + o_map0);
     p.gdata_off = reinterpret_cast<const unsigned long long*>(dp + o_gdata);
     p.goff_base = reinterpret_cast<const unsigned long long*>(dp + o_goff);
+    p.bad = static_cast<unsigned long long*>(d_bad.p);
+    p.n_bad = reinterpret_cast<unsigned long long*>(dp + o_nbad);
     RV_CUDA(cudaEventRecord(ev[0], stream));
     RV_CUDA(cudaMemcpyAsync(dp + o_ids, keys, key_bytes, cudaMemcpyHostToDevice, stream));
     RV_CUDA(cudaMemsetAsync(dp + o_err, 0xFF, 8, stream));
-    launch_versions_partition(p, v->single_object, stream);
+    RV_CUDA(cudaMemsetAsync(dp + o_nbad, 0, 8, stream));
+    launch_versions_partition(p, v->single_object, perm, stream);
     RV_CUDA(cudaGetLastError());
-    std::vector<unsigned long long> back(1 + G * 2);
-    RV_CUDA(cudaMemcpyAsync(back.data(), dp + o_err, back.size() * 8, cudaMemcpyDeviceToHost, stream));  // the err word, then the totals at o_tot
+    std::vector<unsigned long long> back(2 + G * 2);
+    RV_CUDA(cudaMemcpyAsync(back.data(), dp + o_err, back.size() * 8, cudaMemcpyDeviceToHost, stream));  // err, n_bad, then the totals
     RV_CUDA(cudaStreamSynchronize(stream));
     unsigned long long best = back[0];
-    auto cnt = [&](size_t g) { return int64_t(back[1 + 2 * g]); };
-    auto bytes = [&](size_t g) { return int64_t(back[2 + 2 * g]); };
+    const int64_t n_part_bad = int64_t(back[1]);
+    if (n_part_bad > n) return fail(RV_ERR_CUDA, "internal error: more bad messages than messages");
+    auto cnt = [&](size_t g) { return int64_t(back[2 + 2 * g]); };
+    auto bytes = [&](size_t g) { return int64_t(back[3 + 2 * g]); };
+    auto is_bad_group = [&](size_t g) { return perm && int(g % size_t(W1)) == W; };
 
     // ---- every message carries the same registered id: the writer's own decode of the input, no copy, no take
     if (best == ~0ull) {
         for (int w = 0; w < W; ++w) {
             int64_t c = 0;
-            for (int j = 0; j < k; ++j) c += cnt(size_t(j) * W + w);
-            if (c != n) continue;
+            for (int j = 0; j < k; ++j) c += cnt(size_t(j) * W1 + w);
+            if (c != n) continue;  // (a message in the bad group: no writer has them all)
             RV_CUDA(cudaEventRecord(ev[1], stream));
             InputHints h = writer_framing(v, w);
             h.total_bytes = total_bytes;
@@ -2273,7 +2296,7 @@ rv_status decode_versions(const rv_versions* v, const uint8_t* d_data, const int
     for (size_t g = 0; g < G; ++g) {
         gdata_off[g] = data_total;
         goff_base[g] = off_total;
-        if (cnt(g) == 0) continue;
+        if (cnt(g) == 0 || is_bad_group(g)) continue;
         data_total = align_up(data_total + size_t(bytes(g)) + 64, 16);
         off_total += align_up(size_t(cnt(g)) + 1, 2);  // every group's offsets 16-byte aligned
     }
@@ -2283,22 +2306,28 @@ rv_status decode_versions(const rv_versions* v, const uint8_t* d_data, const int
     RV_CUDA(cudaMemcpyAsync(dp + o_goff, goff_base.data(), G * 8, cudaMemcpyHostToDevice, stream));
     p.gdata = static_cast<uint8_t*>(d_gdata.p);
     p.goffs = static_cast<int64_t*>(d_goffs.p);
-    launch_versions_scatter(p, stream);
+    if (perm) {
+        RV_CUDA(d_inv.alloc(std::max<size_t>(off_total, 1) * 8, stream));
+        p.inv = static_cast<int64_t*>(d_inv.p);
+    }
+    launch_versions_scatter(p, perm, stream);
     RV_CUDA(cudaGetLastError());
     RV_CUDA(cudaEventRecord(ev[1], stream));
 
-    // ---- every group through its writer's resolved decode; the lowest failing message of all wins
+    // ---- every group through its writer's resolved decode (permissive: its permissive form, whose bad rows stay in the
+    // group's part); the lowest failing message of all wins
     SubResults subs;
     subs.r.assign(G, nullptr);
+    int64_t n_sub_bad = 0;
     for (size_t g = 0; g < G; ++g) {
-        if (cnt(g) == 0) continue;
-        const int j = int(g / size_t(W)), w = int(g % size_t(W));
+        if (cnt(g) == 0 || is_bad_group(g)) continue;
+        const int j = int(g / size_t(W1)), w = int(g % size_t(W1));
         InputHints h = writer_framing(v, w);
         h.total_bytes = bytes(g);
         unsigned long long ew = ~0ull;
         const rv_status st = decode_on_device(v->writers[size_t(w)], p.gdata + gdata_off[g], p.goffs + goff_base[g], cnt(g), 1, h, stream,
                                               device, &subs.r[g], 0, &ew);
-        if (!st) continue;
+        if (!st) { n_sub_bad += int64_t(subs.r[g]->bad_records.size()); continue; }
         if (ew == ~0ull) return st;  // not an error of a message
         int64_t msg = 0;
         const rv_status st2 = global_index(p.map0, int64_t(j) * chunk_rows, j == k - 1 ? last_rows : chunk_rows, w, int64_t(ew >> 8), stream, &msg);
@@ -2315,14 +2344,7 @@ rv_status decode_versions(const rv_versions* v, const uint8_t* d_data, const int
             RV_CUDA(cudaStreamSynchronize(stream));
             RV_CUDA(cudaMemcpyAsync(hdr, d_data + a, v->single_object ? kSingleObjectHeader : 5, cudaMemcpyDeviceToHost, stream));
             RV_CUDA(cudaStreamSynchronize(stream));
-            if (v->single_object) {
-                uint64_t fp = 0;
-                for (int b = 0; b < 8; ++b) fp |= uint64_t(hdr[2 + b]) << (8 * b);
-                return fail(RV_ERR_FRAME, "single-object message: schema fingerprint " + hex_fingerprint(fp) + " is not registered (record " +
-                                              std::to_string(rec) + ")");
-            }
-            const uint32_t id = (uint32_t(hdr[1]) << 24) | (uint32_t(hdr[2]) << 16) | (uint32_t(hdr[3]) << 8) | uint32_t(hdr[4]);
-            return fail(RV_ERR_FRAME, "framed message: schema id " + std::to_string(id) + " is not registered (record " + std::to_string(rec) + ")");
+            return fail(RV_ERR_FRAME, unregistered_text(v, hdr) + " (record " + std::to_string(rec) + ")");
         }
         const char* text = code == E_FRAME && v->single_object ? kSingleObjectFrameText : err_text(code);
         return fail(status_of(code), std::string(text) + " (record " + std::to_string(rec) + ")");
@@ -2335,7 +2357,7 @@ rv_status decode_versions(const rv_versions* v, const uint8_t* d_data, const int
     std::vector<unsigned long long> chunk_tot(size_t(k) * size_t(S1), 0ull);
     for (int j = 0; j < k; ++j) {
         for (int w = 0; w < W; ++w) {
-            const rv_result* r = subs.r[size_t(j) * W + w];
+            const rv_result* r = subs.r[size_t(j) * W1 + w];
             if (r) parts[size_t(j)][size_t(w)] = VersionPart{&r->chunks[0], static_cast<const uint8_t*>(r->arenas[0]->dev)};
         }
         versions_chunk_totals(rp, v->pairs, parts[size_t(j)], chunk_tot.data() + size_t(j) * size_t(S1));
@@ -2361,9 +2383,34 @@ rv_status decode_versions(const rv_versions* v, const uint8_t* d_data, const int
     RV_CUDA(cudaMemcpyAsync(d_take.p, tp.header.data(), tp.header_bytes, cudaMemcpyHostToDevice, stream));
     for (size_t l = 0; l + 1 < tp.level_first.size(); ++l)
         launch_take_level(tp.spaces + tp.level_first[l], tp.level_first[l + 1] - tp.level_first[l], tp.level_blocks[l], tp.jobs,
-                          tp.scans + tp.scan_first[l], tp.scan_first[l + 1] - tp.scan_first[l], stream);
+                          tp.scans + tp.scan_first[l], tp.scan_first[l + 1] - tp.scan_first[l], perm, stream);
     RV_CUDA(cudaGetLastError());
     RV_CUDA(cudaEventRecord(ev[3], stream));
+    // ---- the report of a permissive call, only when it has bad messages: the sub-decodes' group rows appended to the
+    // partition's list, mapped to messages on the device with the E_FRAME_ID headers, one read-back
+    std::vector<unsigned long long> bad_words;
+    std::vector<uint8_t> bad_hdr;
+    const int64_t n_bad = n_part_bad + n_sub_bad;
+    if (n_bad > n) return fail(RV_ERR_CUDA, "internal error: more bad messages than messages");
+    if (n_bad > 0) {
+        std::vector<unsigned long long> sub_words;
+        sub_words.reserve(size_t(n_sub_bad));
+        for (size_t g = 0; g < G; ++g)
+            if (subs.r[g])
+                for (size_t i = 0; i < subs.r[g]->bad_records.size(); ++i)
+                    sub_words.push_back((static_cast<unsigned long long>(goff_base[g] + uint64_t(subs.r[g]->bad_records[i])) << 8) |
+                                        subs.r[g]->bad_codes[i]);
+        RV_CUDA(d_hdr.alloc(size_t(n_bad) * 16, stream));
+        if (!sub_words.empty())
+            RV_CUDA(cudaMemcpyAsync(p.bad + n_part_bad, sub_words.data(), sub_words.size() * 8, cudaMemcpyHostToDevice, stream));
+        launch_versions_report(p.bad, n_part_bad, n_bad, p.inv, d_data, d_offsets, v->single_object ? int(kSingleObjectHeader) : 5,
+                               static_cast<uint8_t*>(d_hdr.p), stream);
+        RV_CUDA(cudaGetLastError());
+        bad_words.resize(size_t(n_bad));
+        bad_hdr.resize(size_t(n_bad) * 16);
+        RV_CUDA(cudaMemcpyAsync(bad_words.data(), p.bad, size_t(n_bad) * 8, cudaMemcpyDeviceToHost, stream));
+        RV_CUDA(cudaMemcpyAsync(bad_hdr.data(), d_hdr.p, size_t(n_bad) * 16, cudaMemcpyDeviceToHost, stream));
+    }
     RV_CUDA(cudaStreamSynchronize(stream));
     guard.armed = false;
     cudaEventElapsedTime(&t_vtimings[0], ev[0], ev[1]);
@@ -2373,7 +2420,23 @@ rv_status decode_versions(const rv_versions* v, const uint8_t* d_data, const int
 
     auto res = std::make_unique<rv_result>();
     res->schema = rv_schema_retain(v->reader);
-    for (int j = 0; j < k; ++j) versions_null_counts(rp, v->pairs, parts[size_t(j)], L.chunks[size_t(j)]);
+    for (int j = 0; j < k; ++j)
+        versions_null_counts(rp, v->pairs, parts[size_t(j)], L.chunks[size_t(j)], perm ? cnt(size_t(j) * W1 + W) : 0);
+    if (n_bad > 0) {
+        // message order, each with the strict call's message minus "(record N)"
+        std::map<int64_t, std::string> id_text;
+        for (size_t i = 0; i < bad_words.size(); ++i)
+            if ((bad_words[i] & 0xFF) == E_FRAME_ID) id_text[int64_t(bad_words[i] >> 8)] = unregistered_text(v, bad_hdr.data() + i * 16);
+        sort_bad_words(bad_words, n);
+        res->single_object = v->single_object;
+        for (unsigned long long w : bad_words) {
+            const int64_t m = int64_t(w >> 8);
+            const uint32_t code = uint32_t(w & 0xFF);
+            res->bad_records.push_back(m);
+            res->bad_codes.push_back(code == E_FRAME_ID ? uint32_t(E_FRAME) : code);
+            res->bad_texts.push_back(code == E_FRAME_ID ? id_text[m] : std::string(code == E_FRAME && v->single_object ? kSingleObjectFrameText : err_text(code)));
+        }
+    }
     res->chunks = std::move(L.chunks);
     res->arenas.assign(res->chunks.size(), arena_sp);
     res->arrow_bytes = exported_bytes(rp, res->chunks);
@@ -2496,6 +2559,32 @@ rv_status rv_versions_create_single_object(const rv_schema* reader, const rv_sch
     return register_writers(reader, writers, order, columns, n_columns, std::move(v), out);
 }
 
+rv_status rv_versions_permissive(const rv_versions* v, rv_versions** out) {
+    if (!v || !out) return fail(RV_ERR_INVALID, "null argument");
+    *out = nullptr;
+    if (v->permissive) return fail(RV_ERR_INVALID, "rv_versions_permissive: the registry is already permissive");
+    auto p = std::make_unique<rv_versions>();
+    p->single_object = v->single_object;
+    p->ids = v->ids;
+    p->fps = v->fps;
+    p->permissive = true;
+    rv_status st = rv_schema_permissive(v->reader, &p->reader);
+    if (st) return st;
+    for (size_t i = 0; i < v->writers.size(); ++i) {
+        const std::string who = v->single_object ? "writer fingerprint " + hex_fingerprint(v->fps[i]) + ": " : "schema id " + std::to_string(v->ids[i]) + ": ";
+        rv_schema* w = nullptr;
+        st = rv_schema_permissive(v->writers[i], &w);
+        if (st) return fail(st, who + t_error);
+        p->writers.push_back(w);
+        try {
+            p->pairs.push_back(pair_plans(p->reader->plan, w->plan));
+        } catch (const std::exception& e) {
+            return fail(RV_ERR_SCHEMA, who + e.what());
+        }
+    }
+    *out = p.release();
+    return RV_OK;
+}
 
 void rv_versions_release(rv_versions* v) { delete v; }
 

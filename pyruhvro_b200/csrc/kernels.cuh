@@ -45,9 +45,13 @@ void launch_ocf_offsets(const OcfParams& q, cudaStream_t s);
 void launch_gather_push(const PushJob* jobs, int n_jobs, int parts, cudaStream_t s);
 // multi-version Confluent decode (versions.cu): count + scan of the partition, then (after the host placed the groups)
 // the scatter; one level of row spaces of the take
-void launch_versions_partition(const VersionsParams& p, bool single_object, cudaStream_t s);  // keys: p.ids, or p.fps
-void launch_versions_scatter(const VersionsParams& p, cudaStream_t s);
+// keys: p.ids, or p.fps; permissive: the *_perm instances (a bad group per chunk, a null row per kNoRow entry)
+void launch_versions_partition(const VersionsParams& p, bool single_object, bool permissive, cudaStream_t s);
+void launch_versions_scatter(const VersionsParams& p, bool permissive, cudaStream_t s);
 void launch_take_level(const TakeSpace* spaces, int n_spaces, long long blocks, const TakeJob* jobs, const TakeScan* scans, int n_scans,
-                       cudaStream_t s);
+                       bool permissive, cudaStream_t s);
+// permissive registries: the call's bad list in message terms, and the headers of its E_FRAME_ID messages (16 bytes each)
+void launch_versions_report(unsigned long long* list, int64_t n_part, int64_t n, const int64_t* inv, const uint8_t* data, const int64_t* offsets,
+                            int header_bytes, uint8_t* hdr, cudaStream_t s);
 
 }  // namespace rv

@@ -19,7 +19,8 @@ namespace rv {
 
 constexpr int kMaxVersions = 256;   // registered writer schemas of one rv_versions handle (the partition's id table)
 constexpr uint32_t E_FRAME_ID = 14; // framed message whose schema id / fingerprint is not registered (reported as RV_ERR_FRAME)
-constexpr unsigned long long kNoRow = ~0ull;  // row-map entry of a message that failed its header check
+constexpr unsigned long long kNoRow = ~0ull;  // row-map entry of a message that failed its header check (permissive
+                                              // registries: a null row, rv_versions_permissive)
 
 // A row-map entry: output row -> (writer index, row within that writer's part of the chunk).
 RV_HD unsigned long long take_pack(uint32_t writer, uint64_t row) { return (static_cast<unsigned long long>(writer) << 40) | row; }
@@ -113,6 +114,11 @@ struct VersionsParams {
     const unsigned long long* goff_base; // [k][W] where group g's rows + 1 offsets start in goffs
     unsigned long long* map0;            // [n] space-0 row map (take_pack)
     const unsigned long long* fps;       // [W] single-object registries: the writers' fingerprints, ascending (instead of ids)
+    // permissive registries only: the tables above have W + 1 columns (n_ids = W + 1), the last being every chunk's
+    // bad group (framing errors and unregistered keys: no bytes, no sub-decode, a kNoRow row-map entry)
+    unsigned long long* bad;             // [n] (message << 8 | code) of the bad-group messages
+    unsigned long long* n_bad;           // their count
+    int64_t* inv;                        // [goffs entries] group row -> message (the inverse of the row map)
 };
 
 // Validity / Bits: the source row's bit (a missing validity buffer counts as all valid).
@@ -156,6 +162,19 @@ RV_HD void take_offsets_row(const TakeJob& j, uint32_t w, int64_t s, int64_t r, 
         const int64_t first = take_start(j, w, s);
         for (int32_t q = 0; q < len; ++q) j.child_map[pos + q] = take_pack(w, uint64_t(first + q));
     }
+}
+
+// A null row of a permissive registry (row-map entry kNoRow): what a permissive decode writes for a bad record.  Bits
+// and validity are 0 (take_rows_kernel), fixed-width values and N-variant union type ids 0, offsets open no items or
+// bytes and start no rows in any child row space.
+RV_HD void take_null_value(const TakeJob& j, int64_t r) {
+    uint8_t* dst = j.dst + r * j.width;
+    for (int i = 0; i < j.width; ++i) dst[i] = 0;
+}
+RV_HD void take_null_offsets_row(const TakeJob& j, int64_t r, int32_t pos) {
+    int32_t* o = reinterpret_cast<int32_t*>(j.dst);
+    o[r + 1] = pos;
+    if (r == 0) o[0] = 0;
 }
 
 // Per-lane copy of one row's bytes: 8-byte words where source and destination agree mod 8, else bytes.

@@ -82,9 +82,10 @@ void versions_chunk_totals(const Plan& reader, const std::vector<VersionPairing>
     }
 }
 
-void versions_null_counts(const Plan& reader, const std::vector<VersionPairing>& pairs, const std::vector<VersionPart>& parts, ChunkOut& out) {
+void versions_null_counts(const Plan& reader, const std::vector<VersionPairing>& pairs, const std::vector<VersionPart>& parts, ChunkOut& out,
+                          int64_t null_rows) {
     for (int sl : reader.validity_slots) {
-        int64_t nulls = 0;
+        int64_t nulls = reader.slots[size_t(sl)].space == 0 ? null_rows : 0;
         for (size_t w = 0; w < parts.size(); ++w)
             if (parts[w].c && pairs[w].slot[size_t(sl)] >= 0) nulls += parts[w].c->null_count[size_t(pairs[w].slot[size_t(sl)])];
         out.null_count[size_t(sl)] = nulls;

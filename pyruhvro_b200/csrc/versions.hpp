@@ -33,10 +33,12 @@ struct VersionPart {
 };
 
 // The take permutes rows inside a chunk, so the chunk's row counts, stream totals and null counts are the sums over its
-// parts.  tot: the chunk's row of compute_layout's chunk_tot ([max(S, 1)] reader streams).
+// parts.  tot: the chunk's row of compute_layout's chunk_tot ([max(S, 1)] reader streams).  null_rows: the chunk's bad
+// group of a permissive registry, rows of space 0 that add to no stream and are null in every space-0 validity bitmap.
 void versions_chunk_totals(const Plan& reader, const std::vector<VersionPairing>& pairs, const std::vector<VersionPart>& parts,
                            unsigned long long* tot);
-void versions_null_counts(const Plan& reader, const std::vector<VersionPairing>& pairs, const std::vector<VersionPart>& parts, ChunkOut& out);
+void versions_null_counts(const Plan& reader, const std::vector<VersionPairing>& pairs, const std::vector<VersionPart>& parts, ChunkOut& out,
+                          int64_t null_rows = 0);
 
 // The job tables of one take, laid out for a scratch block at `base` (device memory, or host memory in the emulation):
 // [header: spaces, jobs, scans, pointer tables][block sums][child row maps].  `header` is the image of the first
